@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- DMRG sweep wall-clock and effective-H matvec throughput, 1..N B200 vs the reference CPU path.
+"""bench.py -- DMRG sweep wall-clock and effective-H matvec throughput, 1..N H100 vs the reference CPU path.
 
 Workload (BASELINE.json configs[1]): TFIChain L=100, two-site DMRG at chi=1024, no charge conservation
 (dense-block path).  One *step* = one full DMRG sweep = 2(L-2) = 196 two-site bond updates through
@@ -16,6 +16,11 @@ N > 1 (launched by torchrun): the path shards over independent DMRG runs (a fiel
 configs[4]); rank r runs the same workload at g = 1 + 0.02 r, the only collectives are an NCCL broadcast of
 the model template and an all-gather of the per-run results; ``value`` = max-over-ranks sweep time / N
 (seconds per sweep of the whole job, weak scaling).
+
+``--dump-outputs DIR`` writes what the last timed sweep computed, as a caller of the sweep receives it, to DIR/*.npy
+(float64): the energy, the Schmidt values and entanglement entropies of every bond and a fixed, seeded sample of the
+entries of every MPS tensor.  The inputs are seeded, so two builds run with the same arguments can be compared output
+for output.
 """
 import argparse
 import json
@@ -33,19 +38,7 @@ if ROOT not in sys.path:
 
 METRIC = 'dmrg_two_site_sweep_wall_clock'
 UNIT = 's'
-FP64_TENSOR_PEAK_TFLOPS = 37.0   # B200 (HGX) FP64 tensor/DFMA spec; MEASURED_PEAKS.json has no FP64 entry
-
-
-def gemm_ncu_numbers():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch and tensor-pipe activity of the matvec GEMM kernel,
-    taken from the committed ncu --set full summary (profiles/gemm_ncu.json, written from the capture named in it);
-    ``(None, None, None)`` if no capture of the current kernel configuration is committed."""
-    path = os.path.join(ROOT, 'profiles', 'gemm_ncu.json')
-    if not os.path.exists(path):
-        return None, None, None
-    with open(path) as f:
-        d = json.load(f)
-    return d.get('dram_bytes_per_launch'), d.get('tensor_pipe_active_pct'), d.get('source')
+FP64_TENSOR_PEAK_TFLOPS = 67.0   # H100 SXM FP64 tensor-core data-sheet figure (700 W); MEASURED_PEAKS.json has no FP64 entry
 
 
 def parse_args():
@@ -79,7 +72,12 @@ def parse_args():
                     help='BASELINE.json configs[4]: chi in {256,512,1024,2048} x two fields, sharded over the ranks by LPT '
                          '(tenpy_b200.scan); auto = on for N > 1')
     ap.add_argument('--scan-chis', default='256,512,1024,2048')
-    return ap.parse_args()
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the results of the last timed sweep to DIR/<name>.npy (see the module doc string)')
+    args = ap.parse_args()
+    if args.dump_outputs and 'reference' in (args.impl, args.driver):
+        ap.error('--dump-outputs writes what the GPU arm computed: not available with --impl reference / --driver reference')
+    return args
 
 
 def measured_peaks():
@@ -87,7 +85,7 @@ def measured_peaks():
         with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as f:
             return json.load(f), 'measured'
     except Exception:
-        return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0}, 'fallback'
+        return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'fallback'     # H100 SXM data sheet (dense, 700 W)
 
 
 # ------------------------------------------------------------------------------------------ clocks sampler
@@ -514,6 +512,34 @@ def psi_from_host(psi, host_bufs):
     return nbytes
 
 
+DUMP_SAMPLE_PER_TENSOR = 8192
+DUMP_SEED = 20261015
+
+
+def _host_f64(x):
+    return (x.detach().cpu().numpy() if hasattr(x, 'detach') else np.asarray(x)).astype(np.float64).ravel()
+
+
+def dump_outputs(dirname, psi, E):
+    """--dump-outputs: energy, Schmidt values and entanglement entropies of every bond, and DUMP_SAMPLE_PER_TENSOR entries
+    of every MPS tensor at positions drawn from a generator seeded per site (the same positions in every run of the same
+    shapes); at most L * 64 KB of samples, 6.5 MB at L = 100."""
+    os.makedirs(dirname, exist_ok=True)
+    L = len(psi._B)
+    sample = []
+    for i in range(L):
+        dense = _host_f64(psi.get_B(i).to_ndarray())
+        rng = np.random.default_rng([DUMP_SEED, i])
+        idx = np.sort(rng.choice(dense.size, size=min(dense.size, DUMP_SAMPLE_PER_TENSOR), replace=False))
+        sample.append(dense[idx])
+    out = {'energy': np.array([E], dtype=np.float64),
+           'schmidt_values': np.concatenate([_host_f64(S) for S in psi._S]),
+           'entanglement_entropy': _host_f64(psi.entanglement_entropy()),
+           'mps_tensor_sample': np.concatenate(sample)}
+    for name, a in out.items():
+        np.save(os.path.join(dirname, name + '.npy'), a)
+
+
 def run_b200(args):
     import torch
     import torch.distributed as dist
@@ -572,6 +598,8 @@ def run_b200(args):
     barrier()
     launches = lib.kernel_launch_count()
     ms = ev0.elapsed_time(ev1) / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, psi, float(eng.update_stats['E_total'][-1]))
     clocks = sampler.summary() if rank == 0 else None
     E_final = eng.update_stats['E_total'][-1]
     S_mid = eng._entropy_approx[L // 2]
@@ -687,7 +715,7 @@ def run_b200(args):
     dominant = max(shares, key=shares.get) if shares else 'gemm'
     roofline = roof['svd'] if dominant == 'svd' else roof['gemm']
     roofline = dict(roofline)
-    roofline['kernel'] = 'jacobi_gram/eig/apply_kernel (block SVD)' if dominant == 'svd' else 'oz_gemm_kernel (matvec, tcgen05 kind::i8)'
+    roofline['kernel'] = 'jacobi_gram/eig/apply_kernel (block SVD)' if dominant == 'svd' else roof['gemm']['kernel'] + ' (matvec)'
     roofline['share_of_step'] = shares.get(dominant)
     if e2e:
         e2e['value'] = float(allst[:, 3].max()) / world
@@ -948,15 +976,15 @@ def kernel_probes(lib, chi, d, D):
     vL, vR, lp = (npc.LegCharge.from_trivial(chi, ci, +1), npc.LegCharge.from_trivial(chi, ci, -1),
                   npc.LegCharge.from_trivial(d, ci, +1))
     theta = rnd([lL, lR])
-    # the two large products of the matvec as the sweep runs them (identity-environment route): the D - 1 non-identity
-    # components of LP onto theta and the W0 W1 . theta intermediate onto those of RP, on the int8 tensor path with 7 digit
-    # planes (csrc/ozaki.cu); the digit planes of LP / RP are cached per bond, those of theta / the intermediate are
-    # produced by the split kernels once per matvec (timed separately: `split_ms_per_operand`)
+    # the two large products of the matvec (identity-environment route): the D - 1 non-identity components of LP onto theta
+    # and the W0 W1 . theta intermediate onto those of RP, timed on both kernels that can run them -- the DMMA grouped GEMM
+    # and the int8 tensor path with 7 digit planes (csrc/ozaki.cu, operands pre-split as in the sweep, split timed
+    # separately); the roofline reports the one npc.OZAKI['enabled'] selects
     from tenpy_b200.linalg.np_conserved import OZAKI
     s7 = int(OZAKI['slices_matvec'])
     Dr = max(D - 1, 1)
     shapes = [(chi * Dr, d * d * chi, chi), (chi * d * d, chi, chi * Dr)]      # (m, n, k)
-    ops, ms_mm, ms_split = [], [], []
+    ops, ms_mm, ms_split, ms_dmma = [], [], [], []
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     reps = 10
     for (m_, n_, k_) in shapes:
@@ -980,6 +1008,15 @@ def kernel_probes(lib, chi, d, D):
         ev1.record()
         torch.cuda.synchronize()
         ms_split.append(ev0.elapsed_time(ev1) / reps)
+        gg = [np.array([m_]), np.array([n_]), np.array([0]), np.array([0, 1]), np.array([k_]), np.array([0]), np.array([0])]
+        lib.grouped_gemm(*gg, A, B, C)
+        ev0.record()
+        for _ in range(reps):
+            lib.grouped_gemm(*gg, A, B, C)
+        ev1.record()
+        torch.cuda.synchronize()
+        ms_dmma.append(ev0.elapsed_time(ev1) / reps)
+        lib.ozaki_mm(m_, n_, k_, s7, a_s, b_s, C, n_)
         ops.append((A, B, C))
     lib.ozaki_check_abort()
     # parity of the timed kernel at the timed size (size-independent property: linearity in a random probe vector,
@@ -992,27 +1029,22 @@ def kernel_probes(lib, chi, d, D):
     scale = A.view(m_, k_).abs() @ (B.view(k_, n_).abs() @ x.abs())
     oz_err = float(((lhs - rhs).abs() / scale).max())
     del ops
-    ms = float(np.mean(ms_mm))
     flops = 2. * Dr * d**2 * chi**3                  # per launch (FP64-equivalent)
     n_prod = s7 * (s7 + 1) // 2                      # exact int8 slice products per FP64 product
-    tf = flops / (ms * 1e-3) / 1e12
-    traffic, pipe_pct, ncu_src = gemm_ncu_numbers() if (chi, d, D) == (1024, 2, 3) else (None, None, None)
-    int8_peak = 2. * peaks.get('bf16_tflops', 0.)    # tcgen05 kind::i8 runs at twice the bf16 rate
-    peak_equiv = int8_peak / n_prod
-    gemm = {'bound': 'tensor', 'achieved': tf, 'peak': peak_equiv, 'unit': 'TFLOP/s', 'frac': tf / peak_equiv if peak_equiv else None,
-            'traffic': traffic, 'ms_per_launch': ms, 'ms_per_launch_by_shape': {'%dx%dx%d' % sh: t for sh, t in zip(shapes, ms_mm)},
-            'int8_tops_achieved': tf * n_prod, 'int8_tops_peak': int8_peak, 'frac_of_nominal_int8_4500': tf * n_prod / 4500., 'digit_planes': s7, 'int8_products_per_fp64_product': n_prod,
-            'split_ms_per_operand': float(np.mean(ms_split)),
-            'fp64_dmma_peak_tflops': FP64_TENSOR_PEAK_TFLOPS, 'frac_of_fp64_dmma_peak': tf / FP64_TENSOR_PEAK_TFLOPS,
-            'algorithmic_bytes_per_launch': float(s7 * (shapes[0][0] * shapes[0][2] + shapes[0][1] * shapes[0][2]) + 8 * shapes[0][0] * shapes[0][1]),
-            'tensor_pipe_active_pct_ncu': pipe_pct, 'ncu_source': ncu_src, 'rel_err_vs_fp64_probe': oz_err,
-            'peak_note': 'achieved = FP64-equivalent flops (2 m n k) per launch / CUDA-event time of oz_gemm_kernel alone, operands pre-split '
-                         'as in the sweep; peak = int8 tensor peak / %d slice products, int8 peak = 2 x bf16_tflops of MEASURED_PEAKS.json '
-                         '(%.0f TFLOP/s %s, burst) = %.0f Top/s (nominal 4500; MMA-only ceiling of this tile shape measured by '
-                         'profiles/tc_i8_probe.cu: 4000-4540); the FP64 tensor (DMMA) pipe the round-1 kernel ran on peaks at %.0f TFLOP/s'
-                         % (n_prod, peaks.get('bf16_tflops', 0.), kind, int8_peak, FP64_TENSOR_PEAK_TFLOPS),
-            'algorithmic': '2 (D-1) d^2 chi^3 = %.3e FP64-equivalent flop per launch = %.3e int8 op: (chi (D-1) x chi).(chi x d^2 chi) and '
-                           '(chi d^2 x chi (D-1)).(chi (D-1) x chi), the two large products of one matvec' % (flops, flops * n_prod)}
+    int8_peak = 2. * peaks.get('bf16_tflops', 0.)    # dense int8 wgmma runs at twice the bf16 rate
+    tf_oz, tf_dmma = flops / (np.mean(ms_mm) * 1e-3) / 1e12, flops / (np.mean(ms_dmma) * 1e-3) / 1e12
+    int8 = {'kernel': 'oz_gemm_kernel', 'achieved': tf_oz, 'peak': int8_peak / n_prod, 'digit_planes': s7,
+            'ms_per_launch_by_shape': {'%dx%dx%d' % sh: t for sh, t in zip(shapes, ms_mm)},
+            'split_ms_per_operand': float(np.mean(ms_split)), 'rel_err_vs_fp64_probe': oz_err,
+            'peak_note': 'int8 tensor peak (2 x bf16_tflops, %s) / %d slice products' % (kind, n_prod)}
+    dmma = {'kernel': 'grouped_gemm_kernel', 'achieved': tf_dmma, 'peak': FP64_TENSOR_PEAK_TFLOPS,
+            'ms_per_launch_by_shape': {'%dx%dx%d' % sh: t for sh, t in zip(shapes, ms_dmma)},
+            'peak_note': 'FP64 tensor-core data-sheet figure'}
+    sel = dict(int8 if OZAKI['enabled'] else dmma)
+    gemm = dict(sel, bound='tensor', unit='TFLOP/s', frac=sel['achieved'] / sel['peak'] if sel['peak'] else None,
+                traffic=None, ms_per_launch=float(np.mean(ms_mm if OZAKI['enabled'] else ms_dmma)), int8_path=int8,
+                dmma_path=dmma, algorithmic='2 (D-1) d^2 chi^3 = %.3e FP64-equivalent flop per launch: (chi (D-1) x chi).'
+                '(chi x d^2 chi) and (chi d^2 x chi (D-1)).(chi (D-1) x chi), the two large products of one matvec' % flops)
     # SVD of the centre theta: bytes = 8 (mn + mk + k + kn)
     from tenpy_b200.linalg.np_conserved import svd
     svd(theta)
@@ -1151,6 +1183,8 @@ def run_blocksparse(args):
     launches = lib.kernel_launch_count()
     sweep_s = ev0.elapsed_time(ev1) / 1e3 / args.steps
     clocks = sampler.summary()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, psi, float(eng.update_stats['E_total'][-1]))
     # one more sweep with per-call profiling
     lib.profile = {}
     plans0 = len(npc._PLAN_CACHE)

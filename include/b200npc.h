@@ -1,4 +1,4 @@
-/* b200npc.h -- C ABI of libb200npc.so, the sm_100a device library behind tenpy_b200.
+/* b200npc.h -- C ABI of libb200npc.so, the sm_90a device library behind tenpy_b200.
  *
  * This is the drop-in boundary for the two-site-DMRG hot path of tenpy/tenpy.  Each entry point
  * replaces one piece of the reference's native helper `tenpy/linalg/_npc_helper.pyx` (the only
@@ -105,7 +105,7 @@ int b200_grouped_gemm_f64(int64_t n_tasks, const int64_t *m_host, const int64_t 
                           const int64_t *k_host, const int64_t *a_off_host, const int64_t *b_off_host,
                           const double *A, const double *B, double *C, b200_stream_t stream);
 
-/* ---- FP64 products on the int8 tensor path (tcgen05.mma kind::i8, accumulators in tensor memory) --------------------- */
+/* ---- FP64 products on the int8 tensor path (wgmma s8 x s8, int32 accumulators in registers) --------------------- */
 /* Ozaki splitting: each operand is cut into `slices` signed 7-bit digit planes (row-wise power-of-two scaling), the slice
  * products are exact int8 x int8 -> int32 tensor-core GEMMs fed by bulk async copies (TMA unit), the diagonals are summed
  * in FP64.  slices = 7: error ~1e-14 (|A||B|)_ij (Lanczos matvec), 8: FP64 rounding level.  Used by npc.tensordot for
@@ -153,7 +153,7 @@ int b200_lanczos_update_f64(int64_t n, double alpha, const double *V1, double be
  * beta = sqrt(beta2_dev[0]) (the |w|^2 of the previous step; beta2_dev / V0 may be NULL), and x *= 1/sqrt(norm2_dev[0]).
  * A Lanczos iteration (krylov_based.py:645-676) then needs no host round trip; the (alpha, beta) pairs are read back
  * in chunks for the tridiagonal eigenproblem and the convergence test.  Bit-identical to the host-scalar route.
- * Default since round 2 (sweep L=24 chi=1024: 0.487 -> 0.406 s on the B200); lanczos_params['device_scalars'] = False switches back. */
+ * Default; lanczos_params['device_scalars'] = False switches back. */
 int b200_lanczos_update_dev_f64(int64_t n, const double *alpha_dev, const double *V1, const double *beta2_dev,
                                 const double *V0, double *W, double *scratch_dev, double *out_dev,
                                 b200_stream_t stream);
@@ -184,8 +184,7 @@ int b200_scale_axis_f64(int64_t n_tasks, const int64_t *task_dev, const int64_t 
 /* Batched Householder QR: block i is A_i (m_i x n_i, row-major at A + a_off[i]); Q_i (m_i x k_i, k = min(m, n)) is
  * written to Q + q_off[i], R_i (k_i x n_i, upper triangular, non-negative diagonal) to R + r_off[i].  One CTA per block,
  * one launch, no host round trip.  replaces the per-block np.linalg.qr of npc.qr (np_conserved.py:4139).  `work` =
- * device scratch of b200_block_qr_worksize bytes.  Used for blocks up to 384 rows / columns (np_conserved.qr_method = 'auto':
- * 64x64 0.7 ms vs 17.3 ms of the column-wise Gram-Schmidt, 300x130 17.4 vs 37.5 ms; 512x512 207 vs 150 ms). */
+ * device scratch of b200_block_qr_worksize bytes.  Used for blocks up to 384 rows / columns (np_conserved.qr_method = 'auto'). */
 int64_t b200_block_qr_worksize(int64_t nblocks, const int64_t *m_host, const int64_t *n_host);
 int b200_block_qr_f64(int64_t nblocks, const int64_t *m_host, const int64_t *n_host, const int64_t *a_off_host,
                       const int64_t *q_off_host, const int64_t *r_off_host, const double *A, double *Q, double *R,
@@ -194,8 +193,8 @@ int b200_block_qr_f64(int64_t nblocks, const int64_t *m_host, const int64_t *n_h
 /* OUT[o, n, i] = sum_k M[n, k] T[o, k, i]  (T: outer x K x inner, OUT: outer x N x inner, row-major, i contiguous;
  * M: N x K on the device, K <= 32): a small matrix applied to the middle index without changing the layout.  Fuses the
  * two block transpositions and the skinny GEMM npc.tensordot needs for "W0.W1 applied to LP.theta" in the split-order
- * matvec (TwoSiteH.matvec, reference mps_common.py:1341-1343) into one streaming pass (chi=1024 matvec 1.95 -> 1.69 ms on the
- * B200; default for dense tensors, TwoSiteH.mpo_apply). */
+ * matvec (TwoSiteH.matvec, reference mps_common.py:1341-1343) into one streaming pass (default for dense tensors,
+ * TwoSiteH.mpo_apply). */
 int b200_mid_contract_f64(int64_t K, int64_t N, int64_t outer, int64_t inner, const double *M_dev, const double *T,
                           double *OUT, b200_stream_t stream);
 /* two-segment version: [OUT1; OUT2][o, n, i] = sum_k M[n, k] [T1; T2][o, k, i] with K = K1 + K2 rows taken from T1 then

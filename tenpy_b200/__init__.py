@@ -1,4 +1,4 @@
-"""tenpy_b200 -- a B200-native (sm_100a) block-sparse tensor engine for the two-site DMRG hot path.
+"""tenpy_b200 -- an H100-native (sm_90a) block-sparse tensor engine for the two-site DMRG hot path.
 
 Mirrors the reference interface of tenpy/tenpy for that path (``linalg.np_conserved``, ``linalg.charges``,
 ``linalg.krylov_based``, ``linalg.truncation``, ``algorithms.mps_common.TwoSiteH``, ``algorithms.dmrg``,

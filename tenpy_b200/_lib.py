@@ -1,6 +1,6 @@
 """ctypes binding of ``libb200npc.so`` (the C ABI declared in ``include/b200npc.h``).
 
-There is exactly one compute backend: the CUDA library built from ``tenpy_b200/csrc`` for sm_100a.
+There is exactly one compute backend: the CUDA library built from ``tenpy_b200/csrc`` for sm_90a.
 If the shared object is missing, or no CUDA device is visible, every compute entry point raises
 :class:`B200Error` -- there is deliberately **no** CPU fallback (the CPU restatement of the path lives
 in ``oracle/`` and is test infrastructure only; nothing in this package imports it).
@@ -104,7 +104,7 @@ def load_library(path=None):
     path = path or LIB_PATH
     if not os.path.exists(path):
         raise B200Error("CUDA extension not built: {0} is missing. Run `python -c 'import __graft_entry__ as g; "
-                        "g.build()'` (nvcc, sm_100a). tenpy_b200 has no CPU fallback.".format(path))
+                        "g.build()'` (nvcc, sm_90a). tenpy_b200 has no CPU fallback.".format(path))
     try:
         cdll = ctypes.CDLL(path)
     except OSError as e:
@@ -203,7 +203,7 @@ class TdotPlan:
 class DeviceLib:
     """The (only) compute backend: marshals torch-tensor handles into C-ABI calls."""
 
-    name = 'libb200npc (CUDA sm_100a)'
+    name = 'libb200npc (CUDA sm_90a)'
 
     def __init__(self, path=None):
         import torch
@@ -212,7 +212,7 @@ class DeviceLib:
         if self.c.b200_abi_version() != 1:
             raise B200Error('ABI version mismatch')
         if not torch.cuda.is_available() or self.c.b200_device_count() < 1:
-            raise B200Error('no CUDA device visible: tenpy_b200 computes on a B200 only (no CPU fallback)')
+            raise B200Error('no CUDA device visible: tenpy_b200 computes on an H100 only (no CPU fallback)')
         self.device = torch.device('cuda', torch.cuda.current_device())
         self.profile = None   # set to {} to collect CUDA-event timings per kernel family
         self._stream = None

@@ -1,4 +1,4 @@
-"""Two-site DMRG on the B200-native tensor engine.
+"""Two-site DMRG on the H100-native tensor engine.
 
 Host-side mirror of the reference driver ``tenpy/algorithms/dmrg.py`` (`run` :63, `DMRGEngine` :112,
 `TwoSiteDMRGEngine` :846) and of the sweep logic it inherits from ``mps_common.Sweep`` (:60; `sweep` :345,
@@ -132,8 +132,7 @@ class TwoSiteDMRGEngine:
         self.time0 = time.time()
         self.mixer = None
         # warm start of the Jacobi SVD from the previous update of the same bond (extension, off by default):
-        #   False      : cold start every time (default).  Measured on the B200, XXZ L=100 chi=1024 (profiles/r02j): cold
-        #                3.78 s per sweep, 'full' 3.56 s, 'subspace' 4.02 s; TFI chi=1024: cold is fastest;
+        #   False      : cold start every time (default);
         #   'full'     : rotate theta with the complete previous singular vector bases (keeps 2 (chi d)^2 doubles per bond);
         #   'subspace' : decompose theta inside the span of the previously kept isometry when the part outside is below
         #                the truncation tolerance (truncation.svd_theta); keeps the truncated (U, VH) of every bond.

@@ -190,7 +190,7 @@ class TwoSiteH:
     acts_on = ['vL', 'p0', 'p1', 'vR']
     SPLIT_MIN_BLOCK = 1 << 20
     # 'fused' (default): W0.W1 is applied to LP.theta by the streaming kernel b200_mid_contract(2)_f64 where it applies
-    # (no charges / one block; 1.69 ms instead of 1.95 ms per chi=1024 matvec on the B200, profiles/r02a_optins.md);
+    # (no charges / one block);
     # 'tensordot': always by npc.tensordot (two block transpositions + a skinny GEMM).
     mpo_apply = 'fused'
     # skip the identity components of the environments in the split-order matvec (see _identity_env_setup): host logic on

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers of libb200npc (sm_100a only).
+// common.cuh -- shared helpers of libb200npc (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,6 +1,6 @@
 // gemm.cu -- contraction plans (host) and the grouped FP64 tensor-core GEMM (device).
 //
-// Replaces, for the B200, the reference's `_tensordot_worker` (tenpy/linalg/_npc_helper.pyx:1498):
+// Replaces, on the GPU, the reference's `_tensordot_worker` (tenpy/linalg/_npc_helper.pyx:1498):
 //   * plan construction  <- _tensordot_pre_sort pyx:1337, _tensordot_match_charges pyx:1382,
 //                           packing loop pyx:1710-1754 (host, integers only, cached by the caller)
 //   * grouped GEMM       <- CblasGemmBatch.run pyx:204-274 (level-wise dgemm_batch).  Here every output
@@ -37,7 +37,7 @@ int sm_count() {
             cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess)
             cached = n;
         else
-            return 148;
+            return 132;
     }
     return cached;
 }
@@ -238,7 +238,7 @@ __global__ void __launch_bounds__(WARPS_M *WARPS_N * 32)
 // Contractions over an un-bunched MPO leg (LP.W0 -> LHeff, W1.RP -> RHeff, reference mpo.py:3107-3126) are lists of block
 // products with k = 1 per pair, a handful of pairs per output block and ONE narrow side (n or m of a few elements), the
 // other side being chi_sector^2 long.  A 32 x 32 tensor-core tile computes ~3 % useful work there and the launch has
-// > 10^6 CTAs (measured: 50-110 ms per call at chi = 1024, profiles/r02b).  They are HBM-bound sums of a few scaled
+// > 10^6 CTAs.  They are HBM-bound sums of a few scaled
 // vectors: one thread per element of the long side, the narrow operand read through the read-only path (same address
 // for the whole warp), coalesced on the long operand.
 constexpr int THIN_MAX = 8;      // narrow side <= THIN_MAX elements
@@ -325,10 +325,9 @@ static void build_tiles(const std::vector<GemmTask> &tasks, const std::vector<Ge
         int64_t area128 = cdiv(tk.m, 128) * cdiv(tk.n, 128) * 128 * 128;
         int64_t area64 = cdiv(tk.m, 64) * cdiv(tk.n, 64) * 64 * 64;
         int64_t area32 = cdiv(tk.m, 32) * cdiv(tk.n, 32) * 32 * 32;
-        // 64x64 tiles (4 warps, 4 CTAs/SM) are the default: measured on B200 at the chi=1024 matvec they reach
-        // 31.7 TFLOP/s against 26.8 for 128x128 (8 warps, 1 CTA/SM: fewer resident warps to cover the DMMA
-        // latency, and 768 tiles = 5.19 waves of 148 SMs); see profiles/r01_tile_config.md.  The 128x128 kernel
-        // stays reachable through B200_GEMM_FORCE_CFG=0 for experiments.
+        // 64x64 tiles (4 warps, 4 CTAs/SM) are the default: more resident warps to cover the DMMA latency than
+        // 128x128 (8 warps, 1 CTA/SM); the H100 runs the chi=1024 matvec products on them at 32-41 TFLOP/s (CUDA
+        // events, H100 SXM 80 GB, 700 W).  The 128x128 kernel stays reachable through B200_GEMM_FORCE_CFG=0.
         (void)area128;
         int cfg = 1;
         if (area32 * 10 < area64 * 7) cfg = 2;

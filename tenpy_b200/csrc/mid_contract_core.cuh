@@ -4,7 +4,7 @@
 // This is the step "apply the two-site MPO tensor W0.W1 to LP.theta" of the split-order effective-H matvec
 // (algorithms/mps_common.py TwoSiteH._matvec_split): T = [vR*, (wL p0 p1), vR], M = [(p0' p1' wR), (wL p0 p1)],
 // K = N = D d^2 (12 for the TFI chain).  Through npc.tensordot it costs two 100 MB block transpositions and a skinny
-// GEMM (90 + 91 + 103 us per matvec at chi = 1024, profiles/r01d_launch_shares.md); here T is read once and OUT written
+// GEMM; here T is read once and OUT written
 // once, both coalesced along i, with no change of layout -- the output is exactly the operand the second large GEMM wants.
 // One thread owns one (o, i) column: K loads (stride `inner`), N*K FMAs with M broadcast from shared memory, N stores.
 //

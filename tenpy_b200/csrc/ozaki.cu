@@ -1,5 +1,5 @@
-// ozaki.cu -- FP64 matrix products on the int8 tensor path of the B200 (tcgen05.mma kind::i8, int32 accumulation in
-// tensor memory), for the chi^3 contractions of the effective-H matvec and the environment updates.
+// ozaki.cu -- FP64 matrix products on the int8 tensor path of the H100 (wgmma.mma_async s8 x s8, int32 accumulation in
+// registers), for the chi^3 contractions of the effective-H matvec and the environment updates.
 //
 // Replaces (for large dense blocks) the level-wise dgemm of CblasGemmBatch.run, tenpy/linalg/_npc_helper.pyx:204-274,
 // reached from _tensordot_worker pyx:1498-1790 / np_conserved.py:4846.
@@ -10,20 +10,21 @@
 //   |r| <= 2^(-7 s).  Then
 //       (A B)_ij = 2^(ea_i + eb_j - 12) sum_{d=0}^{s-1} 2^(-7 d) C_d,      C_d = sum_{t+u=d} A_t B_u   (int8 x int8 -> int32)
 //   up to the dropped slice products t + u >= s.  Every C_d is an EXACT integer matrix (k * 2^12 * (d+1) < 2^31), computed
-//   by tcgen05.mma on 128 x 128 tiles with the accumulators in tensor memory; the diagonals are summed in FP64 in the
-//   epilogue.  s = 7 gives ~1e-14 relative to (|A||B|)_ij, s = 8 FP64 rounding level (tests/test_ozaki.py).
+//   by wgmma on 128 x 64 tiles with the accumulators in registers; the diagonals are summed in FP64 in the epilogue.
+//   s = 7 gives ~1e-14 relative to (|A||B|)_ij, s = 8 FP64 rounding level (tests/test_ozaki.py).
 //
 // Data layout.  A split operand ("panel layout") is, per slice t and per tile of 128 rows, the sequence of its 16-byte
 // k-chunks, each chunk stored as 128 rows x 16 bytes (2 KB):   [slice][row tile][k chunk][row in tile][16 B].
 // A stage of the pipeline (4 consecutive k-chunks of one row tile of one slice = 8 KB, contiguous in HBM) is brought in
-// by ONE bulk async copy of the TMA unit (cp.async.bulk, SASS UBLKCP) and is directly the un-swizzled K-major core-matrix
-// layout tcgen05 expects: core matrix (8 rows x 16 B) contiguous, LBO (K direction) = 2048 B, SBO (row direction) = 128 B.
+// by bulk async copies of the TMA unit (cp.async.bulk) and is directly the un-swizzled K-major core-matrix layout wgmma
+// reads: core matrix (8 rows x 16 B) contiguous, LBO (K direction) = chunk stride, SBO (row direction) = 128 B.
 //
-// Kernel (persistent, one CTA per SM, 12 warps): warp 0 = TMA producer, warp 1 = MMA issuer (one thread), warp 2 = TMEM
-// allocation, warps 4..11 = epilogue (TMEM -> registers -> FP64 -> C; two warps per TMEM lane quarter, 64 columns each).  512 TMEM columns = 4 int32 accumulators of
-// 128 x 128, so the diagonals are processed in passes of up to 4, least significant pass first and the groups aligned at the
-// top (s = 7: d = 3..6 then d = 0..2): the last pass needs the fewest slices; within a pass every loaded slice tile is
-// reused by up to 4 MMAs.
+// Kernel (persistent, one CTA per SM, 3 warpgroups): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = MMA
+// and epilogue, each owning 64 rows x 64 columns of the 128 x 64 output tile (the B operand is read as one half of its
+// 128-row panel tile).  A thread holds 4 int32 accumulators of 32 registers, so the diagonals are processed in passes of
+// up to 4, least significant pass first and the groups aligned at the top (s = 7: d = 3..6 then d = 0..2): the last pass
+// needs the fewest slices; within a pass every loaded slice tile is reused by up to 4 MMAs.  The FP64 summation of a pass
+// is the same sequence of operations for every element whatever the tile shape, so results do not depend on it.
 #include <algorithm>
 #include <cstdlib>
 #include <vector>
@@ -295,51 +296,45 @@ struct OzGemmArgs {
     long long *dbg;              // optional (B200_OZ_DEBUG): cycle counters of CTA 0, see b200_ozaki_mm_f64
 };
 
-constexpr int OZ_THREADS = 384;             // warps 0-2: producer / MMA issuer / TMEM allocation, warps 4-11: epilogue
-constexpr int OZ_EPI_THREADS = 256;         // two warps per TMEM lane quarter, 64 columns of the 128 x 128 tile each
+constexpr int OZ_TN = 64;                   // columns of C per CTA tile: one half of a 128-row tile of B
+constexpr int OZ_THREADS = 384;             // warpgroup 0: producer (one thread), warpgroups 1-2: MMA + epilogue
+constexpr int OZ_CONSUMER_THREADS = 256;    // each consumer warpgroup owns 64 rows x 64 columns of the tile
 constexpr int OZ_MAX_STAGES = 4;
 
-__device__ __forceinline__ uint64_t oz_desc(uint32_t saddr) {
-    // un-swizzled K-major: LBO (K direction, between the two 16-byte chunks of an MMA) = 2048 B, SBO (8-row groups) = 128 B
-    return tc05::smem_desc(saddr, OZ_CHUNK_BYTES, 128, 0);
-}
+__device__ __forceinline__ double oz_i2d(uint32_t r) { return (double)(int32_t)r; }
 
 __global__ void __launch_bounds__(OZ_THREADS, 1) oz_gemm_kernel(OzGemmArgs p) {
     extern __shared__ __align__(1024) uint8_t oz_smem[];
-    __shared__ uint64_t full_bar[OZ_MAX_STAGES], empty_bar[OZ_MAX_STAGES], acc_full, acc_empty;
-    __shared__ uint32_t tmem_slot;
-    using namespace tc05;
+    __shared__ uint64_t full_bar[OZ_MAX_STAGES], empty_bar[OZ_MAX_STAGES];
+    using namespace sm90;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int s = p.slices, cps = p.cps, nst = p.nstages;
-    const uint32_t tile_bytes = (uint32_t)cps * OZ_CHUNK_BYTES;       // one slice tile of a stage
-    const uint32_t stage_bytes = 2u * s * tile_bytes;
+    const uint32_t a_bytes = (uint32_t)cps * OZ_CHUNK_BYTES;          // A slice tile of a stage: cps chunks x 128 rows
+    const uint32_t b_bytes = a_bytes / 2;                             // B slice half tile: cps chunks x 64 rows
+    const uint32_t stage_bytes = (uint32_t)s * (a_bytes + b_bytes);
     const int npass = (s + 3) / 4;
     const int ksteps = p.kc / cps;                                    // pipeline stages per pass
-    const int mt_count = (p.M + OZ_TILE - 1) / OZ_TILE, nt_count = (p.N + OZ_TILE - 1) / OZ_TILE;
+    const int mt_count = (p.M + OZ_TILE - 1) / OZ_TILE, nt_count = (p.N + OZ_TN - 1) / OZ_TN;
     const int ntiles = mt_count * nt_count;
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < nst; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
+            mbar_init(&empty_bar[i], OZ_CONSUMER_THREADS);
         }
-        mbar_init(&acc_full, 1);
-        mbar_init(&acc_empty, OZ_EPI_THREADS);
         mbar_fence_init();
     }
-    if (warp == 2) tmem_alloc(&tmem_slot, 512);
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tmem = tmem_slot;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 0) {
+        if (lane != 0) return;
         // ================= producer: bulk copies of slice tiles =================
         uint32_t it = 0;
         bool ok = true;
         long long t_wait = 0, t0 = clock64();
         for (int tile = blockIdx.x; tile < ntiles && ok; tile += gridDim.x) {
             const int mt = tile % mt_count, nt = tile / mt_count;
+            const int bt = nt >> 1, bhalf = nt & 1;
             for (int g = npass - 1; g >= 0 && ok; --g) {
                 const int nsl = s - 4 * (npass - 1 - g);             // slices 0 .. nsl-1 of both operands are needed (= d_hi + 1)
                 for (int ks = 0; ks < ksteps; ++ks, ++it) {
@@ -348,13 +343,17 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) oz_gemm_kernel(OzGemmArgs p) {
                     ok = mbar_wait(&empty_bar[slot], ((it / nst) & 1) ^ 1, p.abort_flag);
                     t_wait += clock64() - tw;
                     if (!ok) break;
-                    mbar_expect_tx(&full_bar[slot], 2u * nsl * tile_bytes);
+                    mbar_expect_tx(&full_bar[slot], (uint32_t)nsl * (a_bytes + b_bytes));
                     uint8_t *st = oz_smem + (size_t)slot * stage_bytes;
                     for (int t = 0; t < nsl; ++t) {
                         const uint8_t *ga = p.As + (((int64_t)t * p.rta + mt) * p.kc + (int64_t)ks * cps) * OZ_CHUNK_BYTES;
-                        const uint8_t *gb = p.Bs + (((int64_t)t * p.rtb + nt) * p.kc + (int64_t)ks * cps) * OZ_CHUNK_BYTES;
-                        bulk_g2s(st + (size_t)t * tile_bytes, ga, tile_bytes, &full_bar[slot]);
-                        bulk_g2s(st + (size_t)(s + t) * tile_bytes, gb, tile_bytes, &full_bar[slot]);
+                        const uint8_t *gb = p.Bs + (((int64_t)t * p.rtb + bt) * p.kc + (int64_t)ks * cps) * OZ_CHUNK_BYTES +
+                                            bhalf * (OZ_CHUNK_BYTES / 2);
+                        bulk_g2s(st + (size_t)t * a_bytes, ga, a_bytes, &full_bar[slot]);
+                        uint8_t *sb = st + (size_t)s * a_bytes + (size_t)t * b_bytes;
+                        for (int c = 0; c < cps; ++c)
+                            bulk_g2s(sb + c * (OZ_CHUNK_BYTES / 2), gb + (size_t)c * OZ_CHUNK_BYTES, OZ_CHUNK_BYTES / 2,
+                                     &full_bar[slot]);
                     }
                 }
             }
@@ -363,142 +362,87 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) oz_gemm_kernel(OzGemmArgs p) {
             p.dbg[0] = clock64() - t0;
             p.dbg[1] = t_wait;
         }
-    } else if (warp == 1 && lane == 0) {
-        // ================= MMA issuer =================
-        const uint32_t idesc = idesc_s8(OZ_TILE, OZ_TILE);
-        uint32_t it = 0, pass_it = 0;
-        bool ok = true;
-        long long t_full = 0, t_acc = 0, t0 = clock64();
-        for (int tile = blockIdx.x; tile < ntiles && ok; tile += gridDim.x) {
-            for (int g = npass - 1; g >= 0 && ok; --g, ++pass_it) {
-                const int d_hi = s - 1 - 4 * (npass - 1 - g), d_lo = max(0, d_hi - 3);
-                long long tw = clock64();
-                ok = mbar_wait(&acc_empty, (pass_it & 1) ^ 1, p.abort_flag);   // epilogue has drained the accumulators
-                t_acc += clock64() - tw;
-                if (!ok) break;
-                fence_after_sync();
-                for (int ks = 0; ks < ksteps; ++ks, ++it) {
-                    const int slot = it % nst;
-                    tw = clock64();
-                    ok = mbar_wait(&full_bar[slot], (it / nst) & 1, p.abort_flag);
-                    t_full += clock64() - tw;
-                    if (!ok) break;
-                    fence_after_sync();
-                    // descriptors of slice tile 0 of A and B in this slot; the other tiles / k-steps differ only in the
-                    // start-address field (bytes >> 4, low bits of the descriptor): one 64-bit add per MMA operand
-                    const uint32_t sa = smem_addr(oz_smem + (size_t)slot * stage_bytes);
-                    const uint64_t da0 = oz_desc(sa), db0 = oz_desc(sa + (uint32_t)s * tile_bytes);
-                    const uint32_t tile16 = tile_bytes >> 4, kstep16 = (2u * OZ_CHUNK_BYTES) >> 4;
-                    for (int d = d_lo; d <= d_hi; ++d) {
-                        const uint32_t acc = tmem + (uint32_t)(d - d_lo) * OZ_TILE;
-                        for (int t = 0; t <= d; ++t) {                 // all pairs (t, u = d - t) of the diagonal
-                            const uint64_t ad = da0 + (uint64_t)((uint32_t)t * tile16);
-                            const uint64_t bd = db0 + (uint64_t)((uint32_t)(d - t) * tile16);
-                            mma_i8(acc, ad, bd, idesc, (ks | t) ? 1u : 0u);
-                            if (cps == 4) mma_i8(acc, ad + kstep16, bd + kstep16, idesc, 1u);
-                        }
-                    }
-                    mma_commit(&empty_bar[slot]);                      // slot free once these MMAs have read it
-                }
-                if (ok) mma_commit(&acc_full);                         // accumulators of this pass complete
-            }
-        }
-        if (p.dbg && blockIdx.x == 0) {
-            p.dbg[2] = clock64() - t0;
-            p.dbg[3] = t_full;
-            p.dbg[4] = t_acc;
-        }
-    } else if (warp >= 4) {
-        // ================= epilogue: TMEM -> FP64 -> C =================
-        const int q = warp & 3;                                        // TMEM lane quarter = warp id % 4
-        const int chalf = (warp - 4) >> 2;                             // columns [64 chalf, 64 chalf + 64) of the tile
-        uint32_t pass_it = 0;
-        bool ok = true;
-        long long t_wait = 0, t0 = clock64();
-        for (int tile = blockIdx.x; tile < ntiles && ok; tile += gridDim.x) {
-            const int mt = tile % mt_count, nt = tile / mt_count;
-            const double *sbp = p.sB + (int64_t)nt * OZ_TILE;
-            for (int g = npass - 1; g >= 0 && ok; --g, ++pass_it) {
-                const int d_hi = s - 1 - 4 * (npass - 1 - g), d_lo = max(0, d_hi - 3);
+        return;
+    }
+    if (warp < 4) return;
+
+    // ================= consumers: wgmma into register accumulators, epilogue straight from the registers =================
+    const int cw = (warp >> 2) - 1;                                   // rows [64 cw, 64 cw + 64) of the 128-row tile
+    const int wl = warp & 3;
+    uint32_t acc[4][32];                                              // one int32 accumulator per diagonal of a pass
+    uint32_t it = 0;
+    bool ok = true;
+    long long t_full = 0, t_epi = 0, t0 = clock64();
+    for (int tile = blockIdx.x; tile < ntiles && ok; tile += gridDim.x) {
+        const int mt = tile % mt_count, nt = tile / mt_count;
+        for (int g = npass - 1; g >= 0 && ok; --g) {
+            const int d_hi = s - 1 - 4 * (npass - 1 - g), d_lo = max(0, d_hi - 3);
+            for (int ks = 0; ks < ksteps; ++ks, ++it) {
+                const int slot = it % nst;
                 const long long tw = clock64();
-                ok = mbar_wait(&acc_full, pass_it & 1, p.abort_flag);
-                t_wait += clock64() - tw;
+                ok = mbar_wait(&full_bar[slot], (it / nst) & 1, p.abort_flag);
+                t_full += clock64() - tw;
                 if (!ok) break;
-                fence_after_sync();
-                // weight of the pass: 2^(-12 - 7 d_lo)
-                const double wpass = __longlong_as_double((long long)(1023 - 12 - 7 * d_lo) << 52);
-                const bool add = (g != npass - 1) || p.accumulate;
-                const int row0 = mt * OZ_TILE + q * 32;                // the 32 rows of this warp
-                const double sa_l = p.sA[row0 + lane];                 // scale of this lane's row (sA is padded to whole tiles)
-                for (int c0 = 64 * chalf; c0 < 64 * chalf + 64; c0 += 32) {
-                    double h[32];
-                    uint32_t r[32];
-                    tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(d_hi - d_lo) * OZ_TILE + c0, r);
-                    tmem_ld_wait();
+                const uint32_t sa = smem_addr(oz_smem + (size_t)slot * stage_bytes) + (uint32_t)cw * 64u * 16u;
+                const uint32_t sb = smem_addr(oz_smem + (size_t)slot * stage_bytes + (size_t)s * a_bytes);
+                wgmma_fence();
+                for (int kk = 0; kk < cps / 2; ++kk) {                // one wgmma covers 32 bytes of K = two chunks
 #pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        h[j] = __hiloint2double(0x43300000, (int)(r[j] ^ 0x80000000u)) - 4503601774854144.0;
-                    for (int d = d_hi - 1; d >= d_lo; --d) {
-                        tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(d - d_lo) * OZ_TILE + c0, r);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            h[j] = fma(h[j], 0.0078125,
-                                       __hiloint2double(0x43300000, (int)(r[j] ^ 0x80000000u)) - 4503601774854144.0);
-                    }
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) h[j] *= sa_l;          // row scale 2^ea_i while lane = row
-                    // (A/B on the B200, r02h: reading the accumulators with the 16x256b fragment shape instead -- 64-byte row
-                    // segments per four threads, no transposition -- made the epilogue 2x SLOWER, 0.339 vs 0.268 ms per
-                    // 2048 x 4096 x 1024 product; this version stays.)
-                    // lane = row, register = column  ->  lane = column, register = row (butterfly transposition with
-                    // static register indices), so that every global access of the warp is one contiguous 256-byte row
-                    // segment of C instead of 32 scattered 8-byte words
-#pragma unroll
-                    for (int b = 16; b >= 1; b >>= 1) {
-                        const bool up = (lane & b) != 0;
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            if ((j & b) == 0) {
-                                const double give = up ? h[j] : h[j | b];
-                                const double got = __shfl_xor_sync(0xffffffffu, give, b);
-                                if (up) h[j] = got; else h[j | b] = got;
-                            }
-                        }
-                    }
-                    const int col = nt * OZ_TILE + c0 + lane;
-                    const double wsb = wpass * sbp[c0 + lane];         // sB is padded to whole tiles
-                    double *cp = p.C + (int64_t)row0 * p.ldc + col;
-                    if (col < p.N) {
-                        if (add) {
-#pragma unroll
-                            for (int j0 = 0; j0 < 32; j0 += 16) {       // 16 row segments in flight (register budget)
-                                double old[16];
-#pragma unroll
-                                for (int j = 0; j < 16; ++j) old[j] = (row0 + j0 + j < p.M) ? cp[(int64_t)(j0 + j) * p.ldc] : 0.0;
-#pragma unroll
-                                for (int j = 0; j < 16; ++j)
-                                    if (row0 + j0 + j < p.M) cp[(int64_t)(j0 + j) * p.ldc] = fma(h[j0 + j], wsb, old[j]);
-                            }
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j)
-                                if (row0 + j < p.M) cp[(int64_t)j * p.ldc] = h[j] * wsb;
+                    for (int j = 0; j < 4; ++j) {
+                        const int d = d_lo + j;
+                        if (d > d_hi) break;
+                        for (int t = 0; t <= d; ++t) {                // all pairs (t, u = d - t) of the diagonal
+                            const uint64_t ad = smem_desc(sa + (uint32_t)t * a_bytes + (uint32_t)kk * 2u * OZ_CHUNK_BYTES,
+                                                          OZ_CHUNK_BYTES, 128);
+                            const uint64_t bd = smem_desc(sb + (uint32_t)(d - t) * b_bytes + (uint32_t)kk * OZ_CHUNK_BYTES,
+                                                          OZ_CHUNK_BYTES / 2, 128);
+                            wgmma_s8_m64n64k32(acc[j], ad, bd, (ks | kk | t) ? 1u : 0u);
                         }
                     }
                 }
-                fence_before_sync();
-                mbar_arrive(&acc_empty);
+                wgmma_commit();
+                wgmma_wait_all();
+                mbar_arrive(&empty_bar[slot]);                        // this thread has finished reading the slot
             }
-        }
-        if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) {
-            p.dbg[5] = clock64() - t0;
-            p.dbg[6] = t_wait;
+            if (!ok) break;
+            // epilogue of the pass: Horner sum of the diagonals in FP64 (weight of the pass 2^(-12 - 7 d_lo)), row and
+            // column scales, C (+)= result
+            const long long te = clock64();
+            const int npd = d_hi - d_lo + 1;
+            const double wpass = __longlong_as_double((long long)(1023 - 12 - 7 * d_lo) << 52);
+            const bool add = (g != npass - 1) || p.accumulate;
+            const int row0 = mt * OZ_TILE + cw * 64 + wl * 16 + (lane >> 2);
+            const double sa_r[2] = {p.sA[row0], p.sA[row0 + 8]};     // sA / sB are padded to whole 128-row tiles
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int col = nt * OZ_TN + 8 * j + 2 * (lane & 3) + e;
+                    if (col >= p.N) continue;
+                    const double wsb = wpass * p.sB[col];
+#pragma unroll
+                    for (int hr = 0; hr < 2; ++hr) {
+                        const int row = row0 + 8 * hr;
+                        if (row >= p.M) continue;
+                        const int i = 4 * j + 2 * hr + e;
+                        double h = 0.0;
+#pragma unroll
+                        for (int q = 3; q >= 0; --q)
+                            if (q < npd) h = (q == npd - 1) ? oz_i2d(acc[q][i]) : fma(h, 0.0078125, oz_i2d(acc[q][i]));
+                        h *= sa_r[hr];
+                        double *cp = p.C + (int64_t)row * p.ldc + col;
+                        *cp = add ? fma(h, wsb, *cp) : h * wsb;
+                    }
+                }
+            }
+            t_epi += clock64() - te;
         }
     }
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem, 512);
+    if (p.dbg && blockIdx.x == 0 && threadIdx.x == 128) {
+        p.dbg[2] = clock64() - t0;
+        p.dbg[3] = t_full;
+        p.dbg[4] = t_epi;
+    }
 }
 
 const bool g_split_fused = getenv("B200_OZ_SPLIT2") == nullptr;   // B200_OZ_SPLIT2=1: the two-pass split kernels (A/B)
@@ -606,10 +550,11 @@ extern "C" int b200_ozaki_mm_f64(int64_t m, int64_t n, int64_t k, int32_t slices
     // pipeline shape: as many k chunks per stage as leave at least two stages in shared memory
     static const int force_cps = getenv("B200_OZ_CPS") ? atoi(getenv("B200_OZ_CPS")) : 0;   // tuning knob (2 or 4)
     p.cps = force_cps == 2 ? 2 : 4;
-    int64_t stage = 2LL * slices * p.cps * OZ_CHUNK_BYTES;
+    // a stage holds, per slice, the A tile (128 rows) and one half of the B tile (64 rows) of cps k chunks
+    int64_t stage = 3LL * slices * p.cps * (OZ_CHUNK_BYTES / 2);
     if (OZ_SMEM_BUDGET / stage < 2) {
         p.cps = 2;
-        stage = 2LL * slices * p.cps * OZ_CHUNK_BYTES;
+        stage = 3LL * slices * p.cps * (OZ_CHUNK_BYTES / 2);
     }
     p.nstages = (int32_t)std::min<int64_t>(OZ_MAX_STAGES, OZ_SMEM_BUDGET / stage);
     if (p.nstages < 1) return set_error(B200_ERR_ARG, "ozaki_mm: too many slices for shared memory");
@@ -619,7 +564,7 @@ extern "C" int b200_ozaki_mm_f64(int64_t m, int64_t n, int64_t k, int32_t slices
         B200_CUDA_CHECK(cudaFuncSetAttribute(oz_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, OZ_SMEM_BUDGET));
         attr_set = true;
     }
-    int64_t ntiles = oz_row_tiles(m) * oz_row_tiles(n);
+    int64_t ntiles = oz_row_tiles(m) * ((n + OZ_TN - 1) / OZ_TN);
     int grid = (int)std::min<int64_t>(ntiles, sm_count());
     oz_gemm_kernel<<<grid, OZ_THREADS, smem, (cudaStream_t)stream>>>(p);
     B200_CHECK_LAUNCH();
@@ -628,8 +573,8 @@ extern "C" int b200_ozaki_mm_f64(int64_t m, int64_t n, int64_t k, int32_t slices
         B200_CUDA_CHECK(cudaMemcpy(h, dbg_dev, sizeof(h), cudaMemcpyDeviceToHost));
         cudaFree(dbg_dev);
         fprintf(stderr, "[oz_gemm m=%lld n=%lld k=%lld s=%d cps=%d stages=%d] CTA0 cycles: producer total %lld wait_empty %lld | "
-                "mma total %lld wait_full %lld wait_acc_empty %lld | epilogue total %lld wait_acc_full %lld\n",
-                (long long)m, (long long)n, (long long)k, slices, p.cps, p.nstages, h[0], h[1], h[2], h[3], h[4], h[5], h[6]);
+                "consumer total %lld wait_full %lld epilogue %lld\n",
+                (long long)m, (long long)n, (long long)k, slices, p.cps, p.nstages, h[0], h[1], h[2], h[3], h[4]);
     }
     return B200_OK;
 }

@@ -1,6 +1,6 @@
 // svd.cu -- batched block-diagonal SVD and symmetric eigen-decomposition by one-sided block Jacobi.
 //
-// Replaces, for the B200, the per-charge-block LAPACK calls of the reference:
+// Replaces, on the GPU, the per-charge-block LAPACK calls of the reference:
 //   npc._svd_worker (tenpy/linalg/np_conserved.py:4950) -> svd_robust.svd (svd_robust.py:37, gesdd/gesvd)
 //   npc._eig_worker (np_conserved.py:5041)              -> np.linalg.eigh (syevd)
 //
@@ -356,8 +356,7 @@ __global__ void __launch_bounds__(JTHREADS)
 
 // Version 3 of the pivot eigen-solver: G and Q live in REGISTERS, rotations go through warp shuffles, shared memory is
 // only the transposition buffer -> two barriers per rotation set and no dependent shared-memory read-modify-write chains
-// (version 1: three barriers and three shared-memory passes per set, 100-116 us per round on the B200 = the latency floor
-// of the whole block SVD, profiles/r01d_launch_shares.md).
+// (version 1: three barriers and three shared-memory passes per set).
 //   thread (warp w, lane l) holds G[l][4w+i] and Q[4w+i][l], i < 4 (256 threads).
 //   one rotation set (16 disjoint pairs (p, q), the same round-robin order as version 1):
 //     1. every lane computes the rotation of the pair its row index l belongs to from sA (= the current G in shared
@@ -808,9 +807,8 @@ __global__ void __launch_bounds__(128)
 
 // ---- host driver -----------------------------------------------------------------------------------
 // pivot eigen-solver: 3 = jacobi_eig_kernel_v3 (registers + shuffles, default), 1 = jacobi_eig_kernel (shared memory).
-// Inner sweeps: ONE inner sweep is faster for generic full-rank blocks (2048^2: 176 -> 145 ms, XXZ-shaped set 40 -> 32 ms,
-// profiles/r02/r02g_svd_variants.jsonl) but the numerically low-rank two-site wave functions of a converged DMRG then
-// need 14 instead of 11 outer sweeps (svd family of the benchmark sweep 718 -> 819 ms, r02h): the default stays 2.
+// Inner sweeps: ONE inner sweep makes a round cheaper, but the numerically low-rank two-site wave functions of a converged
+// DMRG then need more outer sweeps: the default is 2.
 static int g_eig_variant = 3;
 static int env_fused_max_ld() {                     // B200_SVD_FUSED_LD: largest row length of the single-launch rounds (0: off)
     const char *e = getenv("B200_SVD_FUSED_LD");
@@ -818,7 +816,7 @@ static int env_fused_max_ld() {                     // B200_SVD_FUSED_LD: larges
     const int n = atoi(e);
     return n >= 0 ? n : 256;
 }
-static int g_fused_max_ld = env_fused_max_ld();   // measured (r02r): 39 blocks <= 250: 12.8 vs 14.1 ms; one 512^2 block: 26.3 vs 23.2 ms
+static int g_fused_max_ld = env_fused_max_ld();
 static int env_inner_sweeps() {                     // B200_SVD_INNER=0..16 overrides the default (A/B runs of whole sweeps)
     const char *e = getenv("B200_SVD_INNER");
     if (e == nullptr || *e == 0) return J_INNER_SWEEPS;

@@ -1,14 +1,14 @@
-// tc05.cuh -- thin inline-PTX layer over the Blackwell (sm_100a) tensor path used by ozaki.cu:
-// mbarrier, bulk async copies executed by the TMA unit (cp.async.bulk), tensor memory (TMEM) management,
-// tcgen05.mma (kind::i8, int32 accumulation in TMEM), tcgen05.ld for the epilogue.
-// Bit layouts of the shared-memory matrix descriptor and of the instruction descriptor follow the PTX ISA
-// ("tcgen05 matrix descriptors"); the same fields are spelled out in CUTLASS' cute/arch/mma_sm100_desc.hpp.
+// tc05.cuh -- thin inline-PTX layer over the Hopper (sm_90a) tensor path used by ozaki.cu:
+// mbarrier, bulk async copies executed by the TMA unit (cp.async.bulk), warpgroup MMA (wgmma.mma_async, s8 x s8 with
+// int32 accumulation in registers).
+// Bit layout of the shared-memory matrix descriptor follows the PTX ISA ("Matrix Descriptor Format" of the
+// asynchronous warpgroup-level matrix instructions).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 namespace b200 {
-namespace tc05 {
+namespace sm90 {
 
 __device__ __forceinline__ uint32_t smem_addr(const void *p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -18,7 +18,7 @@ __device__ __forceinline__ uint32_t smem_addr(const void *p) {
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(smem_addr(bar)), "r"(count) : "memory");
 }
-// make barrier initialisation visible to the async proxy (TMA unit, tensor core)
+// make barrier initialisation visible to the async proxy (TMA unit)
 __device__ __forceinline__ void mbar_fence_init() {
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
 }
@@ -52,7 +52,7 @@ __device__ __forceinline__ bool mbar_wait(uint64_t *bar, uint32_t parity, volati
     return false;
 }
 
-// ---- bulk async copy global -> shared (TMA unit, SASS UBLKCP), completion on an mbarrier -------------
+// ---- bulk async copy global -> shared (TMA unit), completion on an mbarrier ---------------------------
 __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gsrc, uint32_t bytes, uint64_t *bar) {
     asm volatile(
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(
@@ -60,96 +60,43 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gsrc, uint3
         "l"(gsrc), "r"(bytes), "r"(smem_addr(bar))
         : "memory");
 }
-// generic-proxy writes to shared memory -> visible to the async proxy (tensor core reads)
-__device__ __forceinline__ void fence_proxy_async_smem() {
-    asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-}
 
-// ---- tensor memory ---------------------------------------------------------------------------------
-// one full warp allocates `ncols` (power of two, 32..512) columns; the base address lands in *smem_slot
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_slot, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_addr(smem_slot)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() {
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void fence_after_sync() {
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-}
-
-// ---- descriptors -------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, K-major operand stored as rows of 128 bytes with the 128-byte swizzle
-// (16-byte chunk index XOR (row mod 8)); 8-row groups are 1024 bytes apart (SBO); tile base 1024-byte aligned.
-//   bits [0,14)  start address >> 4          bits [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1)
-//   bits [32,46) stride byte offset >> 4     bits [46,48) version = 1 (sm_100)
-//   bits [61,64) layout: 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// general form (probe): explicit LBO / SBO (bytes) and layout code
-__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
+// ---- shared-memory matrix descriptor ----------------------------------------------------------------
+//   bits [0,14)  start address >> 4     bits [16,30) leading byte offset >> 4 (K direction between core matrices)
+//   bits [32,46) stride byte offset >> 4 (M/N direction between 8-row core matrices)
+//   bits [62,64) layout: 0 = no swizzle (interleaved core matrices of 8 rows x 16 bytes), 1 = 128B, 2 = 64B, 3 = 32B
+__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)(layout & 7) << 61;
     return d;
 }
-// Instruction descriptor for kind::i8: signed 8-bit A and B, both K-major, int32 accumulator, M x N tile.
-//   [4,6) D format (2 = S32)  [7,10) A format (1 = S8)  [10,13) B format (1 = S8)  [15] A major  [16] B major
-//   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t idesc_s8(uint32_t M, uint32_t N) {
-    return (2u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
 
-// ---- MMA issue (one thread), commit, accumulator read-back --------------------------------------------
-// D[tmem] (+)= A[smem] . B[smem]^T   (A: M x 32 bytes of K, B: N x 32 bytes of K per instruction)
-__device__ __forceinline__ void mma_i8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                       uint32_t accumulate) {
+// ---- warpgroup MMA -----------------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
+
+// D (64 x 64, int32, registers of the warpgroup) (+)= A (64 x 32 bytes of K, smem) . B (64 x 32 bytes of K, smem)^T,
+// both operands signed 8-bit and K-major.  Fragment of D held by thread (warp w, lane l) of the warpgroup:
+//   d[4j + 0] = D[16w + l/4][8j + 2(l%4)]      d[4j + 1] = D[16w + l/4][8j + 2(l%4) + 1]
+//   d[4j + 2] = D[16w + l/4 + 8][8j + 2(l%4)]  d[4j + 3] = D[16w + l/4 + 8][8j + 2(l%4) + 1]      (j = 0..7)
+__device__ __forceinline__ void wgmma_s8_m64n64k32(uint32_t (&d)[32], uint64_t a_desc, uint64_t b_desc,
+                                                   uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on `bar` once all previously issued MMAs of this thread have completed (implies fence::before_thread_sync)
-__device__ __forceinline__ void mma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_addr(bar))
-                 : "memory");
-}
-// warp-collective: lane t of the warp receives 32 consecutive columns of TMEM lane (lane base of taddr) + t
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
         "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p;\n\t}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]),
+          "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]),
+          "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]),
+          "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
         : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
 
-// byte offset of element (row r, k-byte kb) inside a 128-byte-swizzled K-major tile (rows of 128 bytes)
-__host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t r, uint32_t kb) {
-    return r * 128u + ((((kb >> 4) ^ (r & 7u)) & 7u) << 4) + (kb & 15u);
-}
-
-}  // namespace tc05
+}  // namespace sm90
 }  // namespace b200

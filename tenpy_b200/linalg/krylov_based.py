@@ -20,7 +20,7 @@ logger = logging.getLogger(__name__)
 
 __all__ = ['KrylovBased', 'LanczosGroundState', 'lanczos']
 
-DEVICE_SCALARS_DEFAULT = True    # Lanczos option `device_scalars`: (alpha, beta) stay on the device, read back in chunks (B200: sweep 0.49 -> 0.41 s at L=24 chi=1024, profiles/r02a_optins.md)
+DEVICE_SCALARS_DEFAULT = True    # Lanczos option `device_scalars`: (alpha, beta) stay on the device, read back in chunks
 
 
 class KrylovBased:

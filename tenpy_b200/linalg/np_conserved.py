@@ -1,4 +1,4 @@
-"""B200-native block-sparse (abelian charge conserving) tensors: the ``np_conserved`` interface.
+"""H100-native block-sparse (abelian charge conserving) tensors: the ``np_conserved`` interface.
 
 Host-side mirror of the reference module ``tenpy/linalg/np_conserved.py`` ("npc"): the class
 :class:`Array` and the functions :func:`tensordot`, :func:`inner`, :func:`norm`, :func:`svd`,
@@ -8,7 +8,7 @@ behaviour, so that DMRG code written against ``npc`` reads the same.  The *imple
 * the blocks of an Array live in ONE packed HBM buffer (:class:`~._layout.BlockLayout`), not in a Python
   list of ndarrays; ``_data`` / ``_qdata`` are materialised on demand for pickling / inspection;
 * charge-sector bookkeeping is integer work on the host producing cached *plans*; all floating point
-  work is done by the sm_100a kernels of ``libb200npc.so`` (grouped FP64 tensor-core GEMM, BLAS-1 passes
+  work is done by the sm_90a kernels of ``libb200npc.so`` (grouped FP64 tensor-core GEMM, BLAS-1 passes
   over the packed buffer, strided block copies, batched block-Jacobi SVD / eigh);
 * there is no CPU code path: without the CUDA extension every operation raises ``B200Error``.
 
@@ -1189,11 +1189,14 @@ def tensordot(a, b, axes=2, _out=None, _oz_slices=None):
     return res
 
 
-# Large dense block products run on the int8 tensor path (tcgen05, csrc/ozaki.cu): FP64 operands are cut into signed
+# Large dense block products can run on the int8 tensor path (wgmma, csrc/ozaki.cu): FP64 operands are cut into signed
 # 7-bit digit planes, the slice products are exact integer tensor-core GEMMs, the result is summed in FP64.  `slices`:
 # 8 = FP64 rounding level (error ~1e-15 (|A||B|)_ij), 7 (~1e-14) inside the Lanczos matvec (TwoSiteH passes
 # `_oz_slices`).  `min_flops` / `min_dim`: below, the DMMA grouped GEMM is as fast and needs no splitting pass.
-OZAKI = {'enabled': True, 'slices': 8, 'slices_matvec': 7, 'min_flops': 2.e9, 'min_dim': 256, 'calls': 0}
+# Off by default: on the H100 the FP64 tensor cores (DMMA, grouped_gemm_kernel) run the matvec products at 32-41 TFLOP/s,
+# the int8 path at 19-22 TFLOP/s FP64-equivalent with 7 digit planes (H100 SXM 80 GB, 700 W, CUDA events, m, n, k from
+# 1024 to 4096).
+OZAKI = {'enabled': False, 'slices': 8, 'slices_matvec': 7, 'min_flops': 2.e9, 'min_dim': 256, 'calls': 0}
 
 
 def _oz_split_operand(lib, arr, role, rows, k, off, slices):
@@ -1662,8 +1665,7 @@ def _fill_null_vectors(lib, m, n, k, r, kf, transposed, bufU, u_off, bufV, v_off
 qr_stats = {'calls': 0, 'columns': 0, 'replaced': 0}   # diagnostics of the Gram-Schmidt QR
 # 'householder': b200_block_qr_f64, one CTA per block, one launch for all blocks; 'cgs2': Gram-Schmidt on the GEMM /
 # BLAS-1 kernels (one host round trip per column); 'auto' (default): Householder for blocks up to QR_HOUSEHOLDER_MAX rows
-# or columns, Gram-Schmidt above.  Measured on the B200 (profiles/r02a_optins.md): 64x64 0.7 ms vs 17.3 ms, 300x130
-# 17.4 vs 37.5 ms, 512x512 207 vs 150 ms.
+# or columns, Gram-Schmidt above.
 qr_method = 'auto'
 QR_HOUSEHOLDER_MAX = 384
 

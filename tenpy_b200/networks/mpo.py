@@ -4,7 +4,7 @@ Minimal mirror of the reference ``tenpy/networks/mpo.py``: `MPO` (:72; tensors `
 ``'wL', 'wR', 'p', 'p*'``, `IdL` / `IdR` indices) and `MPOEnvironment` (:2740) with the four contraction
 routines on the DMRG path -- `_contract_LP` (:3087), `_contract_RP` (:3097), `_contract_LHeff` (:3107),
 `_contract_RHeff` (:3118) -- plus `full_contraction` (:3065).  All `L` environments stay resident in HBM
-(the reference spills them to disk, tools/cache.py; 180 GB make that unnecessary here).
+(the reference spills them to disk, tools/cache.py; 80 GB make that unnecessary here).
 """
 # Copyright (C) 2026 tenpy_b200 authors. Apache-2.0.
 

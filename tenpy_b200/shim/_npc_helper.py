@@ -10,7 +10,7 @@ into ``libb200npc.so`` through the C ABI:
   `LegPipe__init_from_legs`, `_find_row_differences`, `_map_blocks`, `_sliced_copy`,
   `_tensordot_transpose_axes`) run on the host, as they do in the reference's pyx;
 * the floating point workers (`_tensordot_worker`, `_inner_worker`, `Array_iadd_prefactor_other`,
-  `Array_iscale_prefactor`) take the reference Array's HOST blocks, copy them to the device, run the sm_100a
+  `Array_iscale_prefactor`) take the reference Array's HOST blocks, copy them to the device, run the sm_90a
   kernels and copy the result back (this is the ``e2e`` mode: every call pays PCIe; the device-resident
   mirror ``tenpy_b200.linalg.np_conserved`` is the fast path);
 * pure data-movement workers (`Array_itranspose`, `Array__imake_contiguous`, `_combine_legs_worker`,

@@ -1,8 +1,8 @@
 """Checkpoint exchange with the UNMODIFIED reference (SURVEY.md section 8f rank 4): a DMRG state computed by this package
 is converted with `tenpy_b200.tools.interop`, pickled, loaded by stock TeNPy (which measures the same energy and
-continues the run), and a reference state comes back.  Needs the reference (the checkout of the build container or the
-offline install baseline/_ref that travels to the GPU box).  Twice: on the numpy test double (host logic) and, ``-m gpu``, with
-the state computed and re-imported on the B200."""
+continues the run), and a reference state comes back.  Needs the reference ($TENPY_REFERENCE or the copy build()
+places in oracle/_ref); skips without it.  Twice: on the numpy test double (host logic) and, ``-m gpu``, with
+the state computed and re-imported on the GPU."""
 import os
 import subprocess
 import sys
@@ -13,7 +13,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from tenpy_b200 import dropin  # noqa: E402
 
-REF = os.environ.get('TENPY_REFERENCE') or dropin.reference_path() or '/root/reference'
+REF = dropin.reference_path() or ''
 
 SCRIPT = r'''
 import sys, pickle, warnings, io

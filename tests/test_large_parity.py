@@ -68,11 +68,9 @@ def test_large_dmrg_matches_reference(gpu_lib, name):
         # What two converged runs can agree on: a run stopped at dE/|E| < 1e-12 has a state error |d psi|^2 ~ dE / gap ~ 1e-11,
         # i.e. every Schmidt value is determined to ~3e-6 at best (Weyl).  Rounding-level differences between two correct
         # implementations (or two builds of this one) are amplified by the DMRG iteration up to that level in the slowly
-        # converging SU(2) multiplets; measured over five builds on the B200: up to 5.3e-8 for values >= 1e-4, 1.0e-8 for the
-        # MEAN of a degenerate multiplet (the splitting inside a multiplet is convergence noise in both implementations: the
-        # reference's own triplet at bond 10 of the Hubbard run is split by 4e-9), 1.6e-7 in the tail below 1e-4 (weights
-        # 1e-8 .. 1e-14).  Tolerances: 2e-7, 1e-7 and 1e-6 -- a factor of a few above the measured scatter, 3 to 15 times
-        # below the bound.  Energy (1e-10 relative) and all entanglement entropies (1e-8) are asserted above.
+        # converging SU(2) multiplets (the splitting inside a multiplet is convergence noise in both implementations: the
+        # reference's own triplet at bond 10 of the Hubbard run is split by 4e-9).  Tolerances: 2e-7 for values >= 1e-4, 1e-7
+        # for the MEAN of a degenerate multiplet and 1e-6 in the tail, 3 to 15 times below the bound.  Energy (1e-10 relative) and all entanglement entropies (1e-8) are asserted above.
         tol = np.where(ref_i[:n] >= 1.e-4, 2.e-7, 1.e-6)
         assert np.all(np.abs(mine[:n] - ref_i[:n]) <= tol), (i, float(np.max(np.abs(mine[:n] - ref_i[:n]))))
         big = int(np.count_nonzero(ref_i[:n] >= 1.e-4))

@@ -103,6 +103,7 @@ def test_tensordot_int8_route_host_logic(fake_device, monkeypatch):
     from tenpy_b200.models import TFIChain
     from tenpy_b200.networks.mps import MPS
     from tenpy_b200.algorithms import dmrg
+    monkeypatch.setitem(npc.OZAKI, 'enabled', True)
     monkeypatch.setitem(npc.OZAKI, 'min_flops', 0.)
     monkeypatch.setitem(npc.OZAKI, 'min_dim', 2)
     rng = np.random.default_rng(5)
@@ -131,3 +132,22 @@ def test_tensordot_int8_route_host_logic(fake_device, monkeypatch):
     assert fake_device.calls.get('ozaki_mm', 0) > n0
     assert abs(res['E'] - g['tfi_E']) < 1e-10 * abs(g['tfi_E'])
     assert np.max(np.abs(psi.entanglement_entropy() - g['tfi_S'])) < 1e-8
+
+
+@pytest.mark.gpu
+def test_tensordot_int8_route_gpu(gpu_lib, monkeypatch):
+    """npc.tensordot through oz_gemm_kernel when the int8 route is switched on (off by default)"""
+    from tenpy_b200.linalg import np_conserved as npc
+    monkeypatch.setitem(npc.OZAKI, 'enabled', True)
+    monkeypatch.setitem(npc.OZAKI, 'min_flops', 0.)
+    monkeypatch.setitem(npc.OZAKI, 'min_dim', 2)
+    rng = np.random.default_rng(11)
+    a = npc.Array.from_ndarray_trivial(rng.standard_normal((130, 3, 70)), labels=['a', 'b', 'c'])
+    b = npc.Array.from_ndarray_trivial(rng.standard_normal((70, 3, 90)), labels=['c*', 'b*', 'd'])
+    b.legs[0], b.legs[1] = b.legs[0].conj(), b.legs[1].conj()
+    n0 = npc.OZAKI['calls']
+    c = npc.tensordot(a, b, axes=[['c', 'b'], ['c*', 'b*']])
+    gpu_lib.ozaki_check_abort()
+    assert npc.OZAKI['calls'] == n0 + 1
+    ref = np.tensordot(a.to_ndarray(), b.to_ndarray(), axes=[[2, 1], [0, 1]])
+    assert np.max(np.abs(c.to_ndarray() - ref)) < 1e-13 * np.max(np.abs(ref))

@@ -1,26 +1,17 @@
 """`tenpy_b200.linalg.truncation.truncate` (own formulation: conditions on the number of kept values) against the
 reference's `truncate` (truncation.py:146) on randomised spectra and option combinations: same number of kept values, same
-norm, same truncation error.  Needs the reference (baseline/_ref or the checkout); skips otherwise."""
-import os
-import sys
+norm, same truncation error.  The reference's results for these seeded inputs are stored in tests/golden/truncate.npz
+(tests/golden/make_golden_truncate.py)."""
 import warnings
 
 import numpy as np
-import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import helpers as h
 
 
 def test_truncate_matches_reference_randomised():
-    sys.path.insert(0, ROOT)
-    from tenpy_b200 import dropin
     from tenpy_b200.linalg.truncation import truncate as mine
-    path = dropin.reference_path()
-    if path is None or dropin.installed():
-        pytest.skip('plain reference not importable in this process')
-    sys.path.insert(0, path)
-    from tenpy.linalg.truncation import truncate as ref
-    from tenpy.tools.params import Config
+    g = h.load('truncate.npz')
     rng = np.random.default_rng(0)
     with warnings.catch_warnings():
         warnings.simplefilter('ignore')
@@ -47,6 +38,7 @@ def test_truncate_matches_reference_randomised():
                 opts['svd_min'] = float(10 ** rng.uniform(-16, -1)) if rng.random() < .9 else None
             if rng.random() < .7:
                 opts['trunc_cut'] = float(10 ** rng.uniform(-16, -0.5)) if rng.random() < .9 else None
+            assert len(S) == g['n'][trial], trial       # the inputs are the ones the reference saw
             m1, n1, e1 = mine(S, dict(opts))
-            m2, n2, e2 = ref(S, Config(dict(opts), 'trunc'))
-            assert m1.sum() == m2.sum() and abs(n1 - n2) < 1e-14 and abs(e1.eps - e2.eps) < 1e-14, (opts, S)
+            m2, n2, e2 = g['kept'][trial], g['norm'][trial], g['eps'][trial]
+            assert m1.sum() == m2 and abs(n1 - n2) < 1e-14 and abs(e1.eps - e2) < 1e-14, (opts, S)
