@@ -292,6 +292,18 @@ class DeviceLib:
             self._check(self.c.b200_ozaki_mm_f64(int(m), int(n), int(k), int(slices), _ptr(a_split), _ptr(b_split),
                                                  _ptr(C), int(ldc), 1 if accumulate else 0, self.stream()))
 
+    def ozaki_gemm(self, m, n, k, A, lda, B, ldb, C, ldc, slices, accumulate=False):
+        """C (m x n, ldc) (+)= A (m x k, lda) . B (k x n, ldb), all row-major: both splits and the product in one call, the
+        digit planes in a workspace allocated here (include/b200npc.h)"""
+        nbytes = int(self.c.b200_ozaki_gemm_worksize(int(m), int(n), int(k), int(slices)))
+        if nbytes <= 0:
+            raise B200Error('ozaki_gemm: bad shape / slice count')
+        work = self.torch.empty(nbytes, dtype=self.torch.uint8, device=self.device)
+        with _Prof(self, 'gemm', (2. * m * n * k, 1, 1)):
+            self._check(self.c.b200_ozaki_gemm_f64(int(m), int(n), int(k), _ptr(A), int(lda), _ptr(B), int(ldb), _ptr(C),
+                                                   int(ldc), int(slices), 1 if accumulate else 0, _ptr(work), nbytes,
+                                                   self.stream()))
+
     def ozaki_check_abort(self):
         self._check(self.c.b200_ozaki_check_abort())
 

@@ -582,6 +582,9 @@ extern "C" int b200_tdot_plan_create(const int64_t *a_qdata, int64_t n_a, int32_
             delete plan;
             return set_error(B200_ERR_ARG, "inconsistent block sizes within an output block");
         }
+        // an empty product (zero-size contracted block) contributes nothing and must not take a pipeline stage of
+        // grouped_gemm_kernel; its output block stays (a block with no products left is written as zeros)
+        if (a_cols[pr.ai] <= 0) continue;
         GemmPair gp;
         gp.a_off = a_off[pr.ai];
         gp.b_off = b_off[pr.bj];

@@ -1,9 +1,10 @@
 // qr.cu -- batched Householder QR of the charge blocks of a matrix: one CTA per block, one launch per Array.
 //
 // Replaces the per-block LAPACK call of the reference's npc.qr (tenpy/linalg/np_conserved.py:4139, `np.linalg.qr`).
-// Algorithm and phase functions: block_qr_core.cuh (host-checked by tests/csrc/block_qr_host.cpp).  Opt-in until run on
-// a GPU (np_conserved.qr_method = 'householder'); the default npc.qr is a Gram-Schmidt composition of the GEMM / BLAS-1
-// kernels with one host round trip per column.
+// Algorithm and phase functions: block_qr_core.cuh (host-checked by tests/csrc/block_qr_host.cpp; checked on the GPU
+// against LAPACK at edge shapes by tests/test_gpu_kernel_edges.py).  npc.qr uses it for every block of at most 384 rows and
+// columns (np_conserved.qr_method = 'auto', the default; 'householder' sends every block here); larger blocks go to a
+// Gram-Schmidt composition of the GEMM / BLAS-1 kernels.
 #include <algorithm>
 #include <vector>
 

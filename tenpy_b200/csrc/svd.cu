@@ -20,6 +20,7 @@
 #include <chrono>
 #include <cmath>
 #include <cstdlib>
+#include <limits>
 #include <numeric>
 #include <vector>
 
@@ -1192,6 +1193,9 @@ extern "C" int b200_block_svd_f64(int64_t nblocks, const int64_t *m, const int64
                 double fro2 = 0.0;
                 for (int r = 0; r < mt.m; ++r) fro2 += nr[r];
                 mt.defl = g_svd_deflation ? std::max(16.0 * 2.220446049250313e-16 * sqrt((double)mt.p), g_svd_defl_rel) * sqrt(fro2) : 0.0;
+                // an all-zero block: every direction is negligible (norm 0 <= 0), so it is fully deflated (n_act = 0) and
+                // the caller completes both sides; the smallest positive threshold keeps the `defl > 0` bookkeeping on
+                if (g_svd_deflation && fro2 == 0.0) mt.defl = std::numeric_limits<double>::min();
                 changed = true;
             }
             if (mt.m == mt.n) {

@@ -26,7 +26,9 @@ def test_selftest(gpu_lib):
     [(128, 128, 64)], [(300, 200, 100)], [(61, 33, 7), (5, 9, 122), (64, 64, 64)],
     [(1, 1, 1), (3, 1, 5), (17, 31, 2)], [(512, 384, 256), (100, 30, 7)],
     # thin products (un-bunched MPO leg: k = 1, one narrow side): streaming kernels thin_n / thin_m
-    [(5000, 1, 1), (3000, 4, 2), (1, 7000, 1), (3, 2500, 3), (64, 64, 64), (8, 40, 5), (100001, 2, 1)]])
+    [(5000, 1, 1), (3000, 4, 2), (1, 7000, 1), (3, 2500, 3), (64, 64, 64), (8, 40, 5), (100001, 2, 1)],
+    # every n, k (and k // 2 + 1) and offset even: the 16-byte (VEC) variant, at edges that are not multiples of the tile
+    [(66, 34, 2), (18, 22, 10), (130, 98, 34), (6, 194, 66), (200, 130, 130)]])
 def test_grouped_gemm(gpu_lib, shapes):
     from tenpy_b200 import backend
     rng = np.random.default_rng(1)
