@@ -247,6 +247,32 @@ int b200_block_svd_f64(int64_t nblocks, const int64_t *m_host, const int64_t *n_
                        const int64_t *vt_off_host, const double *A, double *U, double *S, double *VT,
                        void *work_dev, int64_t work_bytes, int32_t *info_host, int32_t *nact_host,
                        int32_t *transposed_host, b200_stream_t stream);
+/* Complex counterpart of b200_block_svd_f64: A_i = U_i diag(S_i) VT_i for complex row-major blocks, with the same
+ * shapes, offsets, ordering (S real, descending), synchronous call, info_host, sweep limit and deflation contract
+ * (b200_svd_set_deflation / _set_deflation_tol apply).  PLANAR data: the real and imaginary parts are separate f64
+ * buffers that share one offset table (A_re / A_im at a_off[i], U_re / U_im at u_off[i], VT_re / VT_im at vt_off[i]).
+ * One-sided block Jacobi in complex arithmetic (Gram matrix P P^H, complex 2x2 rotations, real FP64 tensor-core products
+ * on the planes); no block-size limit.  Rank-deficient blocks: as in the real entry, the vectors of the negligible
+ * directions on the non-accumulated side are left ZERO (nact_host / transposed_host say which); the caller completes them
+ * (tenpy_b200.linalg.np_conserved.svd does it with b200_block_qr_z).  Never produces NaN for finite input.
+ * replaces _svd_worker npc:4950 -> svd_robust.svd (LAPACK zgesdd / zgesvd) for complex blocks. */
+int64_t b200_block_svd_z_worksize(int64_t nblocks, const int64_t *m_host, const int64_t *n_host);
+int b200_block_svd_z(int64_t nblocks, const int64_t *m_host, const int64_t *n_host, const int64_t *a_off_host,
+                     const int64_t *u_off_host, const int64_t *s_off_host, const int64_t *vt_off_host,
+                     const double *A_re, const double *A_im, double *U_re, double *U_im, double *S, double *VT_re,
+                     double *VT_im, void *work_dev, int64_t work_bytes, int32_t *info_host, int32_t *nact_host,
+                     int32_t *transposed_host, b200_stream_t stream);
+/* Complex counterpart of b200_block_qr_f64: Householder QR (zgeqr2 + zung2r) of complex row-major blocks, planar buffers
+ * sharing one offset table; Q_i (m_i x k_i) with orthonormal columns, R_i (k_i x n_i) upper triangular with a real
+ * non-negative diagonal.  One CTA per block, one launch, every block size (cost O(m n k) on one SM: meant for the
+ * canonical-form path, not for large dense blocks).  replaces the per-block np.linalg.qr of npc.qr (np_conserved.py:4139)
+ * for complex blocks.  `work` = device scratch of b200_block_qr_z_worksize bytes. */
+int64_t b200_block_qr_z_worksize(int64_t nblocks, const int64_t *m_host, const int64_t *n_host);
+int b200_block_qr_z(int64_t nblocks, const int64_t *m_host, const int64_t *n_host, const int64_t *a_off_host,
+                    const int64_t *q_off_host, const int64_t *r_off_host, const double *A_re, const double *A_im,
+                    double *Q_re, double *Q_im, double *R_re, double *R_im, void *work, int64_t work_bytes,
+                    b200_stream_t stream);
+
 /* Batched symmetric eigen-decomposition of nblocks row-major symmetric matrices A_i (n[i] x n[i]):
  * A_i = V_i diag(W_i) V_i^T, W_i ascending, eigenvectors in the COLUMNS of V_i (row-major n x n).
  * replaces _eig_worker npc:5041 (np.linalg.eigh, LAPACK syevd). */

@@ -80,6 +80,12 @@ _SIGNATURES = {
     'b200_block_svd_worksize': (c_i64, [c_i64, c_i64p, c_i64p]),
     'b200_block_svd_f64': (ctypes.c_int, [c_i64, c_i64p, c_i64p, c_i64p, c_i64p, c_i64p, c_i64p, c_vp, c_vp, c_vp,
                                           c_vp, c_vp, c_i64, c_i32p, c_i32p, c_i32p, c_vp]),
+    'b200_block_svd_z_worksize': (c_i64, [c_i64, c_i64p, c_i64p]),
+    'b200_block_svd_z': (ctypes.c_int, [c_i64, c_i64p, c_i64p, c_i64p, c_i64p, c_i64p, c_i64p, c_vp, c_vp, c_vp, c_vp,
+                                        c_vp, c_vp, c_vp, c_vp, c_i64, c_i32p, c_i32p, c_i32p, c_vp]),
+    'b200_block_qr_z_worksize': (c_i64, [c_i64, c_i64p, c_i64p]),
+    'b200_block_qr_z': (ctypes.c_int, [c_i64, c_i64p, c_i64p, c_i64p, c_i64p, c_i64p, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                       c_vp, c_i64, c_vp]),
     'b200_block_eigh_worksize': (c_i64, [c_i64, c_i64p]),
     'b200_block_eigh_f64': (ctypes.c_int, [c_i64, c_i64p, c_i64p, c_i64p, c_i64p, c_vp, c_vp, c_vp, c_vp, c_i64,
                                            c_i32p, c_vp]),
@@ -407,6 +413,45 @@ class DeviceLib:
                     self.svd_set_deflation(old_defl)
             self._check(rc)
         return info, nact, transp
+
+    def block_svd_z(self, m, n, a_off, u_off, s_off, vt_off, A_re, A_im, U_re, U_im, S, VT_re, VT_im):
+        """complex block SVD on planar buffers (include/b200npc.h); returns (info, nact, transposed) like block_svd"""
+        ms, ns, ao, uo, so, vo = [_i64(x) for x in (m, n, a_off, u_off, s_off, vt_off)]
+        nb = len(ms[0])
+        wbytes = int(self.c.b200_block_svd_z_worksize(nb, ms[1], ns[1]))
+        work = self.torch.empty(wbytes, dtype=self.torch.uint8, device=self.device)
+        info = np.zeros(nb, dtype=np.int32)
+        nact = np.zeros(nb, dtype=np.int32)
+        transp = np.zeros(nb, dtype=np.int32)
+        def call():
+            return self.c.b200_block_svd_z(nb, ms[1], ns[1], ao[1], uo[1], so[1], vo[1], _ptr(A_re), _ptr(A_im), _ptr(U_re),
+                                           _ptr(U_im), _ptr(S), _ptr(VT_re), _ptr(VT_im), _ptr(work), wbytes,
+                                           info.ctypes.data_as(c_i32p), nact.ctypes.data_as(c_i32p),
+                                           transp.ctypes.data_as(c_i32p), self.stream())
+        with _Prof(self, 'svd'):
+            rc = call()
+            if rc == B200_ERR_NOCONV:     # as block_svd: once more with the conservative settings
+                self.noconv_retries += 1
+                old_in, old_defl = self.svd_set_eig_inner_sweeps(4), self.svd_set_deflation(False)
+                try:
+                    for t in (U_re, U_im, VT_re, VT_im):
+                        t.zero_()
+                    rc = call()
+                finally:
+                    self.svd_set_eig_inner_sweeps(old_in)
+                    self.svd_set_deflation(old_defl)
+            self._check(rc)
+        return info, nact, transp
+
+    def block_qr_z(self, m, n, a_off, q_off, r_off, A_re, A_im, Q_re, Q_im, R_re, R_im):
+        """batched complex Householder QR on planar buffers (include/b200npc.h)"""
+        ms, ns, ao, qo, ro = [_i64(x) for x in (m, n, a_off, q_off, r_off)]
+        nb = len(ms[0])
+        wbytes = int(self.c.b200_block_qr_z_worksize(nb, ms[1], ns[1]))
+        work = self.torch.empty(wbytes, dtype=self.torch.uint8, device=self.device)
+        with _Prof(self, 'svd'):
+            self._check(self.c.b200_block_qr_z(nb, ms[1], ns[1], ao[1], qo[1], ro[1], _ptr(A_re), _ptr(A_im), _ptr(Q_re),
+                                               _ptr(Q_im), _ptr(R_re), _ptr(R_im), _ptr(work), wbytes, self.stream()))
 
     def block_qr(self, m, n, a_off, q_off, r_off, A, Q, R):
         """batched Householder QR of the blocks (include/b200npc.h)"""

@@ -54,6 +54,9 @@ struct JMat {
     int32_t n_act;                         // number of non-deflated vectors
     double defl;                           // deflation threshold: rows with norm <= defl are negligible
     double shift;                          // eigh: diagonal shift
+    int64_t yi_off, wi_off;                // complex SVD: imaginary parts of Y and W (planar; y_off / w_off = real parts)
+    double scale;                          // complex SVD: Y = scale * A (a power of two, |scale A|_F ~ 1), S = norms / scale
+    int32_t cplx, pad_;                    // 1: complex matrix (b200_block_svd_z)
 };
 
 constexpr int jacobi_smem_bytes() { return 2 * JP * JLDP * (int)sizeof(double); }   // two panel chunks
@@ -605,10 +608,319 @@ __global__ void __launch_bounds__(JTHREADS)
     jacobi_apply_body(jsmem, work, mats, cta_mat, rmap, round, QTbuf, flags, 0, 1, pair, 1);
 }
 
+// ---- complex one-sided Jacobi (b200_block_svd_z) ---------------------------------------------------
+// Planar data: Y = Yr + i Yi, W = Wr + i Wi.  The same rounds, pairs, convergence test and deflation as the real path;
+// only the arithmetic of the three phases differs:
+//   zjacobi_gram_kernel   G = P P^H:  Re G = Pr Pr^T + Pi Pi^T,  Im G = Pi Pr^T - Pr Pi^T  (four real DMMA products)
+//   zjacobi_eig_kernel    unitary T with T G T^H diagonal by cyclic complex Jacobi rotations: for the pair (p, q) the phase
+//                         e = g_pq / |g_pq| is stripped (row q <- e row q makes g_pq real), then the real rotation of
+//                         (g_pp, g_qq, |g_pq|):  row p <- c x_p - s e x_q,  row q <- s x_p + c e x_q
+//   zjacobi_apply_kernel  P <- T P and W <- T W:  Re = Tr Pr - Ti Pi,  Im = Tr Pi + Ti Pr  (four real DMMA products)
+// Gram partials and T are stored as [real 32x32 | imaginary 32x32] per pair (and split).
+constexpr int ZJ_STAGE = 2 * JP * JLDP;   // doubles of one pipeline stage: real chunk, imaginary chunk
+constexpr int zjacobi_smem_bytes() { return 2 * ZJ_STAGE * (int)sizeof(double); }
+
+__global__ void __launch_bounds__(JTHREADS)
+    zjacobi_gram_kernel(const double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ cta_mat,
+                        const int *__restrict__ rmap, int round, const int *__restrict__ done, double *__restrict__ Gbuf) {
+    extern __shared__ __align__(16) double jsmem[];
+    __shared__ int s_rows[JP];
+    const int split = blockIdx.x, nsplit = gridDim.x, pair = blockIdx.y;
+    const int mi = cta_mat[pair];
+    if (done[mi]) return;
+    const JMat mt = mats[mi];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
+    if (!j_pair_rows(mt, pair - mt.cta_begin, round, rmap, s_rows, tid)) return;
+    __syncthreads();
+    const double *Yr = work + mt.y_off, *Yi = work + mt.yi_off;
+    const int ld = mt.ldy;
+    const int nch = (ld + JKC - 1) / JKC;
+    if (split >= nch) return;
+    const int tm = warp >> 2, tn = warp & 3;  // 2 x 4 tiles of 16 x 8
+    double accr[4] = {0.0, 0.0, 0.0, 0.0}, acci[4] = {0.0, 0.0, 0.0, 0.0};
+    j_load_chunk(jsmem, Yr, ld, s_rows, split * JKC, tid);
+    j_load_chunk(jsmem + JP * JLDP, Yi, ld, s_rows, split * JKC, tid);
+    cp_async_commit();
+    int it = 0;
+    for (int ch = split; ch < nch; ch += nsplit, ++it) {
+        if (ch + nsplit < nch) {
+            double *nxt = jsmem + ((it + 1) & 1) * ZJ_STAGE;
+            j_load_chunk(nxt, Yr, ld, s_rows, (ch + nsplit) * JKC, tid);
+            j_load_chunk(nxt + JP * JLDP, Yi, ld, s_rows, (ch + nsplit) * JKC, tid);
+        }
+        cp_async_commit();
+        cp_async_wait<1>();
+        __syncthreads();
+        const double *sr = jsmem + (it & 1) * ZJ_STAGE, *si = sr + JP * JLDP;
+#pragma unroll 4
+        for (int k8 = 0; k8 < JKC / 8; ++k8) {
+            const int ao = (tm * 16 + g) * JLDP + k8 * 8 + t, bo = (tn * 8 + g) * JLDP + k8 * 8 + t;
+            double ar[4] = {sr[ao], sr[ao + 8 * JLDP], sr[ao + 4], sr[ao + 8 * JLDP + 4]};
+            double ai[4] = {si[ao], si[ao + 8 * JLDP], si[ao + 4], si[ao + 8 * JLDP + 4]};
+            double nar[4] = {-ar[0], -ar[1], -ar[2], -ar[3]};
+            double br[2] = {sr[bo], sr[bo + 4]}, bi[2] = {si[bo], si[bo + 4]};
+            dmma_16x8x8(accr, ar, br);
+            dmma_16x8x8(accr, ai, bi);
+            dmma_16x8x8(acci, ai, br);
+            dmma_16x8x8(acci, nar, bi);
+        }
+        __syncthreads();
+    }
+    cp_async_wait<0>();
+    double *G = Gbuf + ((int64_t)pair * nsplit + split) * (2 * JP * JP);
+    const int r0 = tm * 16 + g, c0 = tn * 8 + 2 * t;
+#pragma unroll
+    for (int part = 0; part < 2; ++part) {
+        const double *acc = part ? acci : accr;
+        double *Gp = G + part * (JP * JP);
+        Gp[r0 * JP + c0] = acc[0];
+        Gp[r0 * JP + c0 + 1] = acc[1];
+        Gp[(r0 + 8) * JP + c0] = acc[2];
+        Gp[(r0 + 8) * JP + c0 + 1] = acc[3];
+    }
+}
+
+__global__ void __launch_bounds__(JTHREADS)
+    zjacobi_eig_kernel(const JMat *__restrict__ mats, const int *__restrict__ cta_mat, int *__restrict__ rot_count,
+                       const int *__restrict__ done, double tol_scale, const double *__restrict__ Gbuf, int nsplit,
+                       double *__restrict__ QTbuf, int *__restrict__ flags, int inner_sweeps) {
+    __shared__ double sGr[JP * JLDG], sGi[JP * JLDG], sTr[JP * JLDG], sTi[JP * JLDG];
+    __shared__ double cs_c[JB], cs_s[JB], cs_er[JB], cs_ei[JB];
+    __shared__ int pr_p[JB], pr_q[JB];
+    __shared__ double red[32];
+    __shared__ int s_rank[JP];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) flags[blockIdx.x] = 0;
+    const int mi = cta_mat[blockIdx.x];
+    if (done[mi]) return;
+    const JMat mt = mats[mi];
+    if (2 * (blockIdx.x - mt.cta_begin) >= mt.nb_act) return;
+    {
+        const int nch = (mt.ldy + JKC - 1) / JKC;
+        const int ns = nsplit < nch ? nsplit : nch;
+        const double *G = Gbuf + (int64_t)blockIdx.x * nsplit * (2 * JP * JP);
+        for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
+            double vr = 0.0, vi = 0.0;
+            for (int sp = 0; sp < ns; ++sp) {
+                vr += G[sp * (2 * JP * JP) + idx];
+                vi += G[sp * (2 * JP * JP) + JP * JP + idx];
+            }
+            const int r = idx / JP, c = idx % JP;
+            sGr[r * JLDG + c] = vr;
+            sGi[r * JLDG + c] = vi;
+            sTr[r * JLDG + c] = (r == c) ? 1.0 : 0.0;
+            sTi[r * JLDG + c] = 0.0;
+        }
+    }
+    __syncthreads();
+
+    // ---- convergence measure of this pair: max |g_rc| / sqrt(g_rr g_cc) over the non-negligible rows ----
+    // (square roots taken separately and hypot below: g_rr g_cc over- or underflows for blocks scaled near 1e+-150)
+    const double defl2 = mt.defl * mt.defl;
+    double offmax = 0.0;
+    for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
+        const int r = idx / JP, c = idx % JP;
+        if (r < c) {
+            const double drr = sGr[r * JLDG + r], dcc = sGr[c * JLDG + c];
+            if (drr > defl2 && dcc > defl2)
+                offmax = fmax(offmax, hypot(sGr[r * JLDG + c], sGi[r * JLDG + c]) / (sqrt(drr) * sqrt(dcc)));
+        }
+    }
+    offmax = warp_max(offmax);
+    if (lane == 0) red[warp] = offmax;
+    __syncthreads();
+    offmax = 0.0;
+#pragma unroll
+    for (int w = 0; w < JTHREADS / 32; ++w) offmax = fmax(offmax, red[w]);
+    const double tol = tol_scale * sqrt((double)mt.p);
+    if (!(offmax > tol)) return;  // uniform for the whole CTA
+    if (tid == 0) atomicAdd(&rot_count[mi], 1);
+
+    // ---- T G T^H diagonal by parallel cyclic complex Jacobi (16 disjoint pairs per rotation set) ----
+    const double tol_in = 1e-15;
+    for (int sweep = 0; sweep < inner_sweeps; ++sweep) {
+        int any = 0;
+        for (int step = 0; step < JP - 1; ++step) {
+            if (tid < JB) {
+                int a, b;
+                if (tid == 0) {
+                    a = JP - 1;
+                    b = step;
+                } else {
+                    a = (step + tid) % (JP - 1);
+                    b = (step - tid + (JP - 1)) % (JP - 1);
+                }
+                const int p = a < b ? a : b, q = a < b ? b : a;
+                const double gpp = sGr[p * JLDG + p], gqq = sGr[q * JLDG + q];
+                const double gr = sGr[p * JLDG + q], gi = sGi[p * JLDG + q];
+                const double ag = hypot(gr, gi);
+                double c = 1.0, s = 0.0, er = 1.0, ei = 0.0;
+                if (gpp > defl2 && gqq > defl2 && ag > tol_in * sqrt(gpp) * sqrt(gqq)) {
+                    er = gr / ag;
+                    ei = gi / ag;
+                    const double aa = gqq - gpp, bb = 2.0 * ag;
+                    const double hh = hypot(aa, bb);
+                    const double tt = (aa >= 0.0) ? bb / (aa + hh) : bb / (aa - hh);
+                    c = rsqrt(1.0 + tt * tt);
+                    s = tt * c;
+                    any = 1;
+                }
+                pr_p[tid] = p;
+                pr_q[tid] = q;
+                cs_c[tid] = c;
+                cs_s[tid] = s;
+                cs_er[tid] = er;
+                cs_ei[tid] = ei;
+            }
+            __syncthreads();
+            // rows of G and T:  row p <- c x_p - s e x_q,  row q <- s x_p + c e x_q
+            for (int idx = tid; idx < 2 * JB * JP; idx += JTHREADS) {
+                const int which = idx / (JB * JP), jj = (idx / JP) % JB, col = idx % JP;
+                double *Xr = which ? sTr : sGr, *Xi = which ? sTi : sGi;
+                const int p = pr_p[jj], q = pr_q[jj];
+                const double c = cs_c[jj], s = cs_s[jj], er = cs_er[jj], ei = cs_ei[jj];
+                const double xpr = Xr[p * JLDG + col], xpi = Xi[p * JLDG + col];
+                const double xqr = Xr[q * JLDG + col], xqi = Xi[q * JLDG + col];
+                const double yr = er * xqr - ei * xqi, yi = er * xqi + ei * xqr;
+                Xr[p * JLDG + col] = c * xpr - s * yr;
+                Xi[p * JLDG + col] = c * xpi - s * yi;
+                Xr[q * JLDG + col] = s * xpr + c * yr;
+                Xi[q * JLDG + col] = s * xpi + c * yi;
+            }
+            __syncthreads();
+            // columns of G (G <- G T^H):  col p <- c y_p - s conj(e) y_q,  col q <- s y_p + c conj(e) y_q
+            for (int idx = tid; idx < JB * JP; idx += JTHREADS) {
+                const int jj = idx / JP, row = idx % JP;
+                const int p = pr_p[jj], q = pr_q[jj];
+                const double c = cs_c[jj], s = cs_s[jj], er = cs_er[jj], ei = cs_ei[jj];
+                const double ypr = sGr[row * JLDG + p], ypi = sGi[row * JLDG + p];
+                const double yqr = sGr[row * JLDG + q], yqi = sGi[row * JLDG + q];
+                const double zr = er * yqr + ei * yqi, zi = er * yqi - ei * yqr;
+                sGr[row * JLDG + p] = c * ypr - s * zr;
+                sGi[row * JLDG + p] = c * ypi - s * zi;
+                sGr[row * JLDG + q] = s * ypr + c * zr;
+                sGi[row * JLDG + q] = s * ypi + c * zi;
+            }
+            __syncthreads();
+        }
+        if (!__syncthreads_or(any)) break;
+    }
+    // rows of T ordered by descending eigenvalue (norm^2), ties by index.  The key is clamped at 0: the rotated diagonal of
+    // a row at rounding level can come out slightly negative and must not sort behind the all-zero padding rows (q..qp-1,
+    // always the last positions of a pair), or the padding content (zero Y, W = a unit vector outside the block) would
+    // move into a real row
+    if (tid < JP) {
+        const double di = fmax(sGr[tid * JLDG + tid], 0.0);
+        int rk = 0;
+        for (int k = 0; k < JP; ++k) {
+            const double dk = fmax(sGr[k * JLDG + k], 0.0);
+            if (dk > di || (dk == di && k < tid)) ++rk;
+        }
+        s_rank[tid] = rk;
+    }
+    __syncthreads();
+    double *QT = QTbuf + (int64_t)blockIdx.x * (2 * JP * JP);
+    for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
+        const int i = idx / JP, k = idx % JP;
+        QT[s_rank[i] * JP + k] = sTr[i * JLDG + k];
+        QT[JP * JP + s_rank[i] * JP + k] = sTi[i * JLDG + k];
+    }
+    if (tid == 0) flags[blockIdx.x] = 1;
+}
+
+// grid (nsplit, pairs, 2): P <- T P (z = 0, rows of Y) and the same rows of W (z = 1)
+__global__ void __launch_bounds__(JTHREADS)
+    zjacobi_apply_kernel(double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ cta_mat,
+                         const int *__restrict__ rmap, int round, const double *__restrict__ QTbuf,
+                         const int *__restrict__ flags) {
+    extern __shared__ __align__(16) double jsmem[];
+    __shared__ int s_rows[JP];
+    const int pair = blockIdx.y;
+    if (!flags[pair]) return;
+    const JMat mt = mats[cta_mat[pair]];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
+    if (!j_pair_rows(mt, pair - mt.cta_begin, round, rmap, s_rows, tid)) return;
+    __syncthreads();
+    const double *QTr = QTbuf + (int64_t)pair * (2 * JP * JP), *QTi = QTr + JP * JP;
+    double qr[2][4][4], qi[2][4][4];
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int k8 = 0; k8 < 4; ++k8) {
+            const int o = (i * 16 + g) * JP + k8 * 8 + t;
+            qr[i][k8][0] = QTr[o];
+            qr[i][k8][1] = QTr[o + 8 * JP];
+            qr[i][k8][2] = QTr[o + 4];
+            qr[i][k8][3] = QTr[o + 8 * JP + 4];
+            qi[i][k8][0] = QTi[o];
+            qi[i][k8][1] = QTi[o + 8 * JP];
+            qi[i][k8][2] = QTi[o + 4];
+            qi[i][k8][3] = QTi[o + 8 * JP + 4];
+        }
+    double *Xr = work + (blockIdx.z ? mt.w_off : mt.y_off);
+    double *Xi = work + (blockIdx.z ? mt.wi_off : mt.yi_off);
+    const int ld = blockIdx.z ? mt.ldw : mt.ldy;
+    const int nch = (ld + JKC - 1) / JKC;
+    const int ch0 = blockIdx.x, chstep = gridDim.x;
+    if (ch0 >= nch) return;
+    j_load_chunk(jsmem, Xr, ld, s_rows, ch0 * JKC, tid);
+    j_load_chunk(jsmem + JP * JLDP, Xi, ld, s_rows, ch0 * JKC, tid);
+    cp_async_commit();
+    int it = 0;
+    for (int ch = ch0; ch < nch; ch += chstep, ++it) {
+        if (ch + chstep < nch) {
+            double *nxt = jsmem + ((it + 1) & 1) * ZJ_STAGE;
+            j_load_chunk(nxt, Xr, ld, s_rows, (ch + chstep) * JKC, tid);
+            j_load_chunk(nxt + JP * JLDP, Xi, ld, s_rows, (ch + chstep) * JKC, tid);
+        }
+        cp_async_commit();
+        cp_async_wait<1>();
+        __syncthreads();
+        const double *sr = jsmem + (it & 1) * ZJ_STAGE, *si = sr + JP * JLDP;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int nt = warp * 2 + h;
+            const int col = ch * JKC + nt * 8;
+            if (col < ld) {
+                double ar[2][4], ai[2][4];
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) ar[i][e] = ai[i][e] = 0.0;
+#pragma unroll
+                for (int k8 = 0; k8 < 4; ++k8) {
+                    const int bo = (k8 * 8 + t) * JLDP + nt * 8 + g;
+                    double br[2] = {sr[bo], sr[bo + 4 * JLDP]}, bi[2] = {si[bo], si[bo + 4 * JLDP]};
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        double nqi[4] = {-qi[i][k8][0], -qi[i][k8][1], -qi[i][k8][2], -qi[i][k8][3]};
+                        dmma_16x8x8(ar[i], qr[i][k8], br);
+                        dmma_16x8x8(ar[i], nqi, bi);
+                        dmma_16x8x8(ai[i], qr[i][k8], bi);
+                        dmma_16x8x8(ai[i], qi[i][k8], br);
+                    }
+                }
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        const int64_t o = (int64_t)s_rows[i * 16 + g + 8 * hh] * ld + col + 2 * t;
+                        *reinterpret_cast<double2 *>(Xr + o) = make_double2(ar[i][2 * hh], ar[i][2 * hh + 1]);
+                        *reinterpret_cast<double2 *>(Xi + o) = make_double2(ai[i][2 * hh], ai[i][2 * hh + 1]);
+                    }
+                }
+            }
+        }
+        __syncthreads();
+    }
+    cp_async_wait<0>();
+}
+
 // ---- init / finalize kernels ---------------------------------------------------------------------
-// squared row norms (first m entries) and column norms (next n entries) of every A: grid (m + n, nmat)
+// squared row norms (first m entries) and column norms (next n entries) of every A: grid (m + n, nmat).
+// Ai (complex input, else NULL): imaginary part, |a|^2 = re^2 + im^2
 __global__ void __launch_bounds__(128) svd_prep_kernel(double *__restrict__ work, const JMat *__restrict__ mats,
-                                                       const double *__restrict__ A) {
+                                                       const double *__restrict__ A, const double *__restrict__ Ai) {
     __shared__ double red[32];
     const JMat mt = mats[blockIdx.y];
     const int v = blockIdx.x;
@@ -619,22 +931,31 @@ __global__ void __launch_bounds__(128) svd_prep_kernel(double *__restrict__ work
         for (int c = threadIdx.x; c < mt.n; c += blockDim.x) {
             double x = a[(int64_t)v * mt.n + c];
             s = fma(x, x, s);
+            if (Ai) {
+                x = Ai[mt.a_off + (int64_t)v * mt.n + c];
+                s = fma(x, x, s);
+            }
         }
     } else {
         const int c = v - mt.m;
         for (int r = threadIdx.x; r < mt.m; r += blockDim.x) {
             double x = a[(int64_t)r * mt.n + c];
             s = fma(x, x, s);
+            if (Ai) {
+                x = Ai[mt.a_off + (int64_t)r * mt.n + c];
+                s = fma(x, x, s);
+            }
         }
     }
     s = block_sum(s, red);
     if (threadIdx.x == 0) work[mt.prep_off + v] = s;
 }
 
-// SVD init: Y[r] = vector perm[r] of A (rows of A, or columns if transposed), zero padded; W = permutation.
-// grid (chunks, nmat)
+// SVD init: Y[r] = vector perm[r] of A (rows of A, or columns if transposed -- not conjugated), zero padded;
+// W = permutation.  Ai (complex input, else NULL): imaginary part into Yi (Wi stays zero).  grid (chunks, nmat)
 __global__ void __launch_bounds__(256) svd_init_kernel(double *__restrict__ work, const JMat *__restrict__ mats,
-                                                       const int *__restrict__ perm, const double *__restrict__ A) {
+                                                       const int *__restrict__ perm, const double *__restrict__ A,
+                                                       const double *__restrict__ Ai) {
     const JMat mt = mats[blockIdx.y];
     double *Y = work + mt.y_off;
     double *W = work + mt.w_off;
@@ -645,8 +966,13 @@ __global__ void __launch_bounds__(256) svd_init_kernel(double *__restrict__ work
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < ny; e += stride) {
         int r = (int)(e / mt.p), c = (int)(e % mt.p);
         int src = pm[r];
-        double v = mt.transposed ? a[(int64_t)c * mt.n + src] : a[(int64_t)src * mt.n + c];
-        Y[(int64_t)r * mt.ldy + c] = v;
+        const int64_t ia = mt.transposed ? (int64_t)c * mt.n + src : (int64_t)src * mt.n + c;
+        if (Ai) {
+            Y[(int64_t)r * mt.ldy + c] = a[ia] * mt.scale;
+            work[mt.yi_off + (int64_t)r * mt.ldy + c] = Ai[mt.a_off + ia] * mt.scale;
+        } else {
+            Y[(int64_t)r * mt.ldy + c] = a[ia];
+        }
     }
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < mt.qp; e += stride)
         W[e * mt.ldw + (e < mt.q ? pm[e] : e)] = 1.0;
@@ -692,6 +1018,10 @@ __global__ void __launch_bounds__(128) jacobi_norms_kernel(double *__restrict__ 
     const double *y = work + mt.y_off + (int64_t)r * mt.ldy;
     double s = 0.0;
     for (int c = threadIdx.x; c < mt.p; c += blockDim.x) s = fma(y[c], y[c], s);
+    if (mt.cplx) {
+        const double *yi = work + mt.yi_off + (int64_t)r * mt.ldy;
+        for (int c = threadIdx.x; c < mt.p; c += blockDim.x) s = fma(yi[c], yi[c], s);
+    }
     s = block_sum(s, red);
     if (threadIdx.x == 0) work[mt.snorm_off + r] = sqrt(s);
 }
@@ -791,6 +1121,44 @@ __global__ void __launch_bounds__(128)
     }
 }
 
+// complex SVD finalize: grid (max_k, nmat).  W Y0 = Y with W unitary and the rows of Y orthogonal:
+//   not transposed (Y0 = A):    A = W^H Y        -> U[:, r] = conj(W[r, :]),  VT[r, :] = Y[r, :] / s_r
+//   transposed (Y0 = A^T):      A = Y^T conj(W)  -> U[:, r] = Y[r, :] / s_r,  VT[r, :] = conj(W[r, :])
+__global__ void __launch_bounds__(128)
+    zsvd_finalize_kernel(const double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ perm,
+                         double *__restrict__ Ur, double *__restrict__ Ui, double *__restrict__ S,
+                         double *__restrict__ VTr, double *__restrict__ VTi) {
+    const JMat mt = mats[blockIdx.y];
+    const int r = blockIdx.x;
+    const int k = mt.q;
+    if (r >= k) return;
+    const int src = perm[mt.perm_off + r];
+    const double s = work[mt.snorm_off + src];
+    const double inv = (s > mt.defl && s > 0.0) ? 1.0 / s : 0.0;   // negligible direction: filled by the caller
+    const double *yr = work + mt.y_off + (int64_t)src * mt.ldy, *yi = work + mt.yi_off + (int64_t)src * mt.ldy;
+    const double *wr = work + mt.w_off + (int64_t)src * mt.ldw, *wi = work + mt.wi_off + (int64_t)src * mt.ldw;
+    if (threadIdx.x == 0) S[mt.s_off + r] = s / mt.scale;     // exact: scale is a power of two
+    if (mt.transposed) {
+        for (int i = threadIdx.x; i < mt.m; i += blockDim.x) {
+            Ur[mt.u_off + (int64_t)i * k + r] = yr[i] * inv;
+            Ui[mt.u_off + (int64_t)i * k + r] = yi[i] * inv;
+        }
+        for (int c = threadIdx.x; c < mt.n; c += blockDim.x) {
+            VTr[mt.vt_off + (int64_t)r * mt.n + c] = wr[c];
+            VTi[mt.vt_off + (int64_t)r * mt.n + c] = -wi[c];
+        }
+    } else {
+        for (int c = threadIdx.x; c < mt.n; c += blockDim.x) {
+            VTr[mt.vt_off + (int64_t)r * mt.n + c] = yr[c] * inv;
+            VTi[mt.vt_off + (int64_t)r * mt.n + c] = yi[c] * inv;
+        }
+        for (int i = threadIdx.x; i < mt.m; i += blockDim.x) {
+            Ur[mt.u_off + (int64_t)i * k + r] = wr[i];
+            Ui[mt.u_off + (int64_t)i * k + r] = -wi[i];
+        }
+    }
+}
+
 // eigh finalize: eigenvalue r (ascending) = norm[perm[r]] - shift; V[:, r] = W[perm[r], :]
 __global__ void __launch_bounds__(128)
     eigh_finalize_kernel(const double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ perm,
@@ -839,7 +1207,9 @@ struct JLayout {
 
 static inline int64_t rup(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 
-static void make_layout(int64_t nblocks, const int64_t *m, const int64_t *n, bool eigh, JLayout &L) {
+// cplx: complex SVD -- Y and W get planar imaginary parts, the Gram partials and Q^T matrices of a pair are complex
+static void make_layout(int64_t nblocks, const int64_t *m, const int64_t *n, bool eigh, JLayout &L, bool cplx = false) {
+    const int64_t cw = cplx ? 2 : 1;
     L.mats.resize((size_t)nblocks);
     int64_t off = 0;
     int cta = 0;
@@ -863,6 +1233,13 @@ static void make_layout(int64_t nblocks, const int64_t *m, const int64_t *n, boo
         off += (int64_t)mt.qp * mt.ldy;
         mt.w_off = off;
         off += (int64_t)mt.qp * mt.ldw;
+        if (cplx) {
+            mt.cplx = 1;
+            mt.yi_off = off;
+            off += (int64_t)mt.qp * mt.ldy;
+            mt.wi_off = off;
+            off += (int64_t)mt.qp * mt.ldw;
+        }
         mt.snorm_off = off;
         off += rup(mt.qp, 16);
         mt.prep_off = off;
@@ -877,13 +1254,14 @@ static void make_layout(int64_t nblocks, const int64_t *m, const int64_t *n, boo
         mt.nb_act = nb;
         mt.n_act = mt.q;
         mt.defl = 0.0;
+        mt.scale = 1.0;
         L.max_q = std::max(L.max_q, (int)mt.q);
         L.max_nb = std::max(L.max_nb, nb);
     }
     L.g_off = off;
-    off += (int64_t)L.cta_mat.size() * J_NSPLIT_MAX * JP * JP;
+    off += (int64_t)L.cta_mat.size() * J_NSPLIT_MAX * JP * JP * cw;
     L.qt_off = off;
-    off += (int64_t)L.cta_mat.size() * JP * JP;
+    off += (int64_t)L.cta_mat.size() * JP * JP * cw;
     L.f64_elems = off;
     L.perm_elems = perm;
     L.rmap_elems = rmap;
@@ -912,7 +1290,8 @@ static void make_layout(int64_t nblocks, const int64_t *m, const int64_t *n, boo
 // directions -- they are moved (logically, through the row map) behind the active rows and never touched
 // again, so a numerically rank-deficient block only iterates on its significant rows.  Active rows are kept
 // ordered by descending norm (de Rijk).
-static int run_jacobi(JLayout &L, char *work, cudaStream_t st, int32_t *info, int max_sweeps) {
+// cplx: the matrices are complex (layout made with cplx = true); the rounds run the zjacobi_* kernels
+static int run_jacobi(JLayout &L, char *work, cudaStream_t st, int32_t *info, int max_sweeps, bool cplx = false) {
     const int nmat = (int)L.mats.size();
     double *wf = reinterpret_cast<double *>(work);
     JMat *d_mats = reinterpret_cast<JMat *>(work + L.off_mats);
@@ -934,6 +1313,10 @@ static int run_jacobi(JLayout &L, char *work, cudaStream_t st, int32_t *info, in
         // (q = 4096: 48 KB of keys and indices + the kernel's static shared memory is above the default limit)
         B200_CUDA_CHECK(cudaFuncSetAttribute(jacobi_reorder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              J_REORDER_MAX * 12));
+        B200_CUDA_CHECK(cudaFuncSetAttribute(zjacobi_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             zjacobi_smem_bytes()));
+        B200_CUDA_CHECK(cudaFuncSetAttribute(zjacobi_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             zjacobi_smem_bytes()));
         attr_set = true;
     }
     std::vector<int> rot((size_t)nmat), done((size_t)nmat, 0);
@@ -972,8 +1355,21 @@ static int run_jacobi(JLayout &L, char *work, cudaStream_t st, int32_t *info, in
         int nsplit = (3 * sm_count() + act_pairs - 1) / std::max(1, act_pairs);
         nsplit = std::max(1, std::min(nsplit, std::min(J_NSPLIT_MAX, (max_ld + JKC - 1) / JKC)));
         // small-block regime: all phases of a round in one launch (one CTA per pair, no column split)
-        const bool fused = g_eig_variant == 3 && max_ld <= g_fused_max_ld;
+        const bool fused = !cplx && g_eig_variant == 3 && max_ld <= g_fused_max_ld;
         for (int r = 0; r < rounds; ++r) {
+            if (cplx) {   // complex: always the three-launch round with column splits
+                zjacobi_gram_kernel<<<dim3((unsigned)nsplit, (unsigned)n_cta), JTHREADS, zjacobi_smem_bytes(), st>>>(
+                    wf, d_mats, d_cta, d_rmap, round_counter, d_done, d_G);
+                B200_CHECK_LAUNCH();
+                zjacobi_eig_kernel<<<n_cta, JTHREADS, 0, st>>>(d_mats, d_cta, d_rot, d_done, tol_scale, d_G, nsplit, d_QT,
+                                                               d_flags, std::max(1, g_eig_inner_sweeps));
+                B200_CHECK_LAUNCH();
+                zjacobi_apply_kernel<<<dim3((unsigned)nsplit, (unsigned)n_cta, 2), JTHREADS, zjacobi_smem_bytes(), st>>>(
+                    wf, d_mats, d_cta, d_rmap, round_counter, d_QT, d_flags);
+                B200_CHECK_LAUNCH();
+                ++round_counter;
+                continue;
+            }
             if (fused) {
                 jacobi_round_fused_kernel<<<n_cta, JTHREADS, jacobi_smem_bytes(), st>>>(
                     wf, d_mats, d_cta, d_rmap, round_counter, d_done, d_rot, tol_scale, d_G, d_QT, d_flags, g_eig_inner_sweeps);
@@ -1146,16 +1542,18 @@ extern "C" int64_t b200_block_svd_worksize(int64_t nblocks, const int64_t *m, co
     return L.total_bytes;
 }
 
-extern "C" int b200_block_svd_f64(int64_t nblocks, const int64_t *m, const int64_t *n, const int64_t *a_off,
-                                  const int64_t *u_off, const int64_t *s_off, const int64_t *vt_off, const double *A,
-                                  double *U, double *S, double *VT, void *work_dev, int64_t work_bytes,
-                                  int32_t *info, int32_t *nact_host, int32_t *transposed_host, b200_stream_t stream) {
+// real (Ai == NULL) and complex (planar: A + i Ai -> U + i Ui, VT + i VTi) block SVD: one host driver
+static int block_svd_impl(int64_t nblocks, const int64_t *m, const int64_t *n, const int64_t *a_off, const int64_t *u_off,
+                          const int64_t *s_off, const int64_t *vt_off, const double *A, const double *Ai, double *U,
+                          double *Ui, double *S, double *VT, double *VTi, void *work_dev, int64_t work_bytes, int32_t *info,
+                          int32_t *nact_host, int32_t *transposed_host, b200_stream_t stream) {
     if (nblocks <= 0) return B200_OK;
     if (nblocks > 65535) return set_error(B200_ERR_ARG, "too many blocks for one SVD batch");
+    const bool cplx = Ai != nullptr;
     cudaStream_t st = (cudaStream_t)stream;
     const double t_start = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
     JLayout L;
-    make_layout(nblocks, m, n, false, L);
+    make_layout(nblocks, m, n, false, L, cplx);
     if (work_bytes < L.total_bytes) return set_error(B200_ERR_ARG, "SVD work buffer too small: %lld < %lld",
                                                      (long long)work_bytes, (long long)L.total_bytes);
     for (int64_t i = 0; i < nblocks; ++i) {
@@ -1179,7 +1577,7 @@ extern "C" int b200_block_svd_f64(int64_t nblocks, const int64_t *m, const int64
         // blocks), vectors ordered by descending norm (de Rijk); both from one pass over A.
         int max_mn = 0;
         for (auto &mt : L.mats) max_mn = std::max(max_mn, mt.m + mt.n);
-        svd_prep_kernel<<<dim3((unsigned)max_mn, (unsigned)nmat), 128, 0, st>>>(wf, d_mats, A);
+        svd_prep_kernel<<<dim3((unsigned)max_mn, (unsigned)nmat), 128, 0, st>>>(wf, d_mats, A, Ai);
         B200_CHECK_LAUNCH();
         std::vector<int> perm0((size_t)L.perm_elems + 1, 0);
         std::vector<double> nr;
@@ -1189,8 +1587,8 @@ extern "C" int b200_block_svd_f64(int64_t nblocks, const int64_t *m, const int64
             nr.resize((size_t)mt.m + mt.n);
             B200_CUDA_CHECK(cudaMemcpyAsync(nr.data(), wf + mt.prep_off, nr.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
             B200_CUDA_CHECK(cudaStreamSynchronize(st));
+            double fro2 = 0.0;
             {
-                double fro2 = 0.0;
                 for (int r = 0; r < mt.m; ++r) fro2 += nr[r];
                 mt.defl = g_svd_deflation ? std::max(16.0 * 2.220446049250313e-16 * sqrt((double)mt.p), g_svd_defl_rel) * sqrt(fro2) : 0.0;
                 // an all-zero block: every direction is negligible (norm 0 <= 0), so it is fully deflated (n_act = 0) and
@@ -1225,6 +1623,13 @@ extern "C" int b200_block_svd_f64(int64_t nblocks, const int64_t *m, const int64
                 mt.nb_act = nb_act;
                 changed = true;
             }
+            // complex: iterate on Y = 2^-e A with |Y|_F ~ 1 (exact).  At |A| ~ 1e-150 the converged off-diagonal Gram
+            // entries would be subnormal (the iteration stops early); at 1e+150 large blocks overflow.  The threshold follows.
+            if (cplx && fro2 > 0.0 && std::isfinite(fro2)) {
+                mt.scale = std::ldexp(1.0, -std::ilogb(std::sqrt(fro2)));
+                if (mt.defl > 0.0) mt.defl *= mt.scale;
+                changed = true;
+            }
         }
         if (changed)
             B200_CUDA_CHECK(cudaMemcpyAsync(work + L.off_mats, L.mats.data(), (size_t)nmat * sizeof(JMat),
@@ -1234,21 +1639,25 @@ extern "C" int b200_block_svd_f64(int64_t nblocks, const int64_t *m, const int64
         int64_t max_elems = 0;
         for (auto &mt : L.mats) max_elems = std::max<int64_t>(max_elems, (int64_t)mt.q * mt.p);
         int64_t gx = std::min<int64_t>(std::max<int64_t>(1, (max_elems + 1023) / 1024), 2048);
-        svd_init_kernel<<<dim3((unsigned)gx, (unsigned)nmat), 256, 0, st>>>(wf, d_mats, d_perm, A);
+        svd_init_kernel<<<dim3((unsigned)gx, (unsigned)nmat), 256, 0, st>>>(wf, d_mats, d_perm, A, Ai);
         B200_CHECK_LAUNCH();
         B200_CUDA_CHECK(cudaStreamSynchronize(st));  // perm0 (host) must outlive the copy
     }
     const bool dbg = getenv("B200_JACOBI_DEBUG") != nullptr;
     auto now = []() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
     const double t_prep = now();
-    int rc = run_jacobi(L, work, st, info, 60);
+    int rc = run_jacobi(L, work, st, info, 60, cplx);
     if (rc) return rc;
     const double t_jac = now();
     std::vector<int> perm;
     rc = sort_norms(L, work, st, false, perm);
     if (rc) return rc;
-    svd_finalize_kernel<<<dim3((unsigned)std::max(1, L.max_q), (unsigned)nmat), 128, 0, st>>>(
-        wf, d_mats, reinterpret_cast<int *>(work + L.off_perm), U, S, VT);
+    if (cplx)
+        zsvd_finalize_kernel<<<dim3((unsigned)std::max(1, L.max_q), (unsigned)nmat), 128, 0, st>>>(
+            wf, d_mats, reinterpret_cast<int *>(work + L.off_perm), U, Ui, S, VT, VTi);
+    else
+        svd_finalize_kernel<<<dim3((unsigned)std::max(1, L.max_q), (unsigned)nmat), 128, 0, st>>>(
+            wf, d_mats, reinterpret_cast<int *>(work + L.off_perm), U, S, VT);
     B200_CHECK_LAUNCH();
     B200_CUDA_CHECK(cudaStreamSynchronize(st));
     if (dbg)
@@ -1261,6 +1670,32 @@ extern "C" int b200_block_svd_f64(int64_t nblocks, const int64_t *m, const int64
     for (int i = 0; i < nmat; ++i)
         if (info[i] < 0) return set_error(B200_ERR_NOCONV, "block Jacobi SVD did not converge for block %d", i);
     return B200_OK;
+}
+
+extern "C" int b200_block_svd_f64(int64_t nblocks, const int64_t *m, const int64_t *n, const int64_t *a_off,
+                                  const int64_t *u_off, const int64_t *s_off, const int64_t *vt_off, const double *A,
+                                  double *U, double *S, double *VT, void *work_dev, int64_t work_bytes,
+                                  int32_t *info, int32_t *nact_host, int32_t *transposed_host, b200_stream_t stream) {
+    return block_svd_impl(nblocks, m, n, a_off, u_off, s_off, vt_off, A, nullptr, U, nullptr, S, VT, nullptr, work_dev,
+                          work_bytes, info, nact_host, transposed_host, stream);
+}
+
+extern "C" int64_t b200_block_svd_z_worksize(int64_t nblocks, const int64_t *m, const int64_t *n) {
+    if (nblocks <= 0) return 256;
+    JLayout L;
+    make_layout(nblocks, m, n, false, L, true);
+    return L.total_bytes;
+}
+
+extern "C" int b200_block_svd_z(int64_t nblocks, const int64_t *m, const int64_t *n, const int64_t *a_off,
+                                const int64_t *u_off, const int64_t *s_off, const int64_t *vt_off, const double *A_re,
+                                const double *A_im, double *U_re, double *U_im, double *S, double *VT_re, double *VT_im,
+                                void *work_dev, int64_t work_bytes, int32_t *info, int32_t *nact_host,
+                                int32_t *transposed_host, b200_stream_t stream) {
+    if (nblocks > 0 && (A_re == nullptr || A_im == nullptr))
+        return set_error(B200_ERR_ARG, "complex SVD: both planes of A are needed");
+    return block_svd_impl(nblocks, m, n, a_off, u_off, s_off, vt_off, A_re, A_im, U_re, U_im, S, VT_re, VT_im, work_dev,
+                          work_bytes, info, nact_host, transposed_host, stream);
 }
 
 extern "C" int64_t b200_block_eigh_worksize(int64_t nblocks, const int64_t *n) {

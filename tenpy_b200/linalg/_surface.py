@@ -6,9 +6,11 @@ states, indexing, sorting of leg charges, element-wise functions, small dense fa
 element by element on the host (``from_ndarray``, ``__setitem__`` of a few numbers), by one host round trip of the small
 tensor involved.  Imported at the end of ``np_conserved.py``, which attaches the methods to :class:`Array`.
 
-`ComplexArray` gives complex128 tensors as a pair of real device Arrays (same legs); every operation is composed of the
-real kernels.  It exists so that the reference's `Site` classes (which always define ``Sy`` & co.) and real-time gates can be
-built; decompositions of complex tensors (svd / eigh / qr) are not provided.
+`ComplexArray` gives complex128 tensors as a pair of real device Arrays (same legs, planar storage); elementwise operations,
+contractions and inner products are composed of the real kernels.  It carries the reference's `Site` operators (``Sy`` & co.)
+and real-time evolution: ``npc.svd`` and ``npc.qr`` of a ComplexArray run the complex block-Jacobi SVD and the complex
+Householder QR kernels (``b200_block_svd_z``, ``b200_block_qr_z``), so the reference's TEBD with ``exp(-i dt H)`` runs on
+the engine.  ``npc.eigh`` of a complex Hermitian matrix is not provided (NotImplementedError).
 """
 import numpy as np
 
@@ -457,16 +459,14 @@ def expm(a):
             pass
     import scipy.linalg
     piped, b = a.as_completely_blocked()
-    dense_blocks = []
-    lay = b._layout if hasattr(b, '_layout') else None
-    if isinstance(b, ComplexArray):
+    if isinstance(b, npc.ComplexArray):       # (the class np_conserved attached, not the placeholder of this module)
         dense = scipy.linalg.expm(b.to_ndarray())
-        res = ComplexArray.from_ndarray(dense, b.legs, qtotal=b.qtotal, cutoff=0., labels=b._labels)
+        res = npc.ComplexArray.from_ndarray(dense, b.legs, qtotal=b.qtotal, cutoff=0., labels=b._labels)
     else:
         if np.any(b.qtotal != 0):
             raise ValueError('expm of a matrix with non-zero total charge')
         blocks = [scipy.linalg.expm(blk) for blk in b.get_blocks_host()]
-        qd = lay.qdata
+        qd = b._layout.qdata
         # blocks that are not stored are zero -> exp = identity on those sectors
         have = set(int(q) for q in qd[:, 0])
         extra_q, extra_b = [], []

@@ -558,6 +558,9 @@ class Array:
         return self.transpose(ref._labels)
 
     def __mul__(self, other):
+        if np.iscomplexobj(other) and np.isscalar(other):     # real Array * complex scalar: a ComplexArray
+            z = complex(other)
+            return ComplexArray(self.copy(deep=True).iscale_prefactor(z.real), self.copy(deep=True).iscale_prefactor(z.imag))
         if np.isscalar(other):
             return self.copy(deep=True).iscale_prefactor(float(other))
         return NotImplemented
@@ -565,6 +568,8 @@ class Array:
     __rmul__ = __mul__
 
     def __imul__(self, other):
+        if np.iscomplexobj(other) and np.isscalar(other):     # changes the type: ``a *= z`` rebinds `a`
+            return self.__mul__(other)
         if np.isscalar(other):
             return self.iscale_prefactor(float(other))
         return NotImplemented
@@ -575,6 +580,8 @@ class Array:
         return NotImplemented
 
     def __itruediv__(self, other):
+        if np.iscomplexobj(other) and np.isscalar(other):
+            return self.__mul__(1.0 / other)
         if np.isscalar(other):
             return self.iscale_prefactor(1.0 / other)
         return NotImplemented
@@ -1303,9 +1310,21 @@ def inner(a, b, axes='labels', do_conj=False):
     """Full contraction ``sum a[i,j,..] b[i,j,..]`` (reference npc:3540; worker pyx:1791).
 
     `axes`: ``'range'`` = leg k of `a` with leg k of `b`; ``'labels'`` (default) = match by label (conjugated
-    labels for ``do_conj=False``); or ``(axes_a, axes_b)``.  ``do_conj=True`` conjugates `a` first."""
+    labels for ``do_conj=False``); or ``(axes_a, axes_b)``.  ``do_conj=True`` conjugates `a` first.
+    With a :class:`ComplexArray` operand the result is a Python ``complex``, composed of the real inner products of the
+    parts."""
     if isinstance(a, list) and isinstance(b, list):
         return sum(inner(w, v, axes=axes, do_conj=do_conj) for w, v in zip(a, b))
+    if isinstance(a, ComplexArray) or isinstance(b, ComplexArray):
+        a_re, a_im = (a.re, a.im) if isinstance(a, ComplexArray) else (a, None)
+        b_re, b_im = (b.re, b.im) if isinstance(b, ComplexArray) else (b, None)
+        sgn = 1. if do_conj else -1.          # conj(a) b = (ar br + ai bi) + i (ar bi - ai br)
+
+        def part(x, y):
+            return 0. if x is None or y is None else float(inner(x, y, axes=axes, do_conj=do_conj))
+        re = part(a_re, b_re) + sgn * part(a_im, b_im)
+        im = part(a_re, b_im) - sgn * part(a_im, b_re)
+        return complex(re, im)
     if a.rank != b.rank:
         raise ValueError('different rank!')
     if axes != 'range':
@@ -1373,6 +1392,8 @@ def trace(a, leg1=0, leg2=1):
     """Trace of a 2D Array (host reduction over the diagonal blocks; cold path)."""
     if a.rank != 2:
         raise NotImplementedError('trace only for rank 2')
+    if isinstance(a, ComplexArray):
+        return complex(trace(a.re, leg1, leg2), trace(a.im, leg1, leg2))
     return float(np.trace(a.to_ndarray()))
 
 
@@ -1415,7 +1436,13 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
     `deflation_tol` (extension, optional): see ``b200_svd_set_deflation_tol`` in include/b200npc.h; ``None``
     keeps the library default (rounding level only, LAPACK-grade factorisation).
     `n_keep` (extension, optional): the caller keeps at most that many singular triplets (``chi_max``); vectors of
-    negligible directions beyond it are not completed (they are zero, their `S` is exactly 0)."""
+    negligible directions beyond it are not completed (they are zero, their `S` is exactly 0).
+
+    A :class:`ComplexArray` `a` is decomposed by the complex block-Jacobi kernel (``b200_block_svd_z``) with the same
+    charges, legs and options; `U` and `VH` are then ComplexArrays and `S` is real.  `guess` is not supported for
+    complex input (NotImplementedError)."""
+    if guess is not None and isinstance(a, ComplexArray):
+        raise NotImplementedError('svd: `guess` (warm start) is only implemented for real Arrays')
     if deflation_tol is None:
         deflation_tol = SVD_DEFAULTS['deflation_tol']        # module-wide default (None: rounding level only)
     if deflation_tol is not None and deflation_tol is not _SVD_LIB_STATE:
@@ -1475,7 +1502,11 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
         raise ValueError('The entries of `qtotal_LR` have to add up to ``a.qtotal``!')
     qtotal_L = chinfo.make_valid(qtotal_L)
     qtotal_R = chinfo.make_valid(qtotal_R)
-    lay = a._layout
+    cplx = isinstance(a, ComplexArray)
+    if cplx:
+        lay, bufA_re, bufA_im = _complex_planes(a)
+    else:
+        lay = a._layout
     if lay.nblocks == 0:
         raise RuntimeError('SVD found no singular values')
     m = lay.shapes[:, 0]
@@ -1500,10 +1531,30 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
     bufU = backend.zeros(lay_U.size)
     bufV = backend.zeros(lay_V.size)
     bufS = backend.empty(int(s_off[-1]))
-    info, nact, transp = lib.block_svd(m, n, lay.offsets, u_off, s_off[:-1], v_off, a._buf, bufU, bufS, bufV)
+    if cplx:
+        bufU_im = backend.zeros(lay_U.size)
+        bufV_im = backend.zeros(lay_V.size)
+        info, nact, transp = lib.block_svd_z(m, n, lay.offsets, u_off, s_off[:-1], v_off, bufA_re, bufA_im, bufU, bufU_im,
+                                             bufS, bufV, bufV_im)
+    else:
+        info, nact, transp = lib.block_svd(m, n, lay.offsets, u_off, s_off[:-1], v_off, a._buf, bufU, bufS, bufV)
     svd_stats['calls'] += 1
     svd_stats['jacobi_sweeps'].append(int(np.max(info)))
-    if np.any(nact < k):
+    if cplx and np.any(nact < k):
+        # complete the zero vectors of the negligible directions in complex arithmetic (QR kernel, cannot fail)
+        S_h = backend.to_host(bufS).copy()
+        for i in np.nonzero(nact < k)[0]:
+            k_fill = int(k[i]) if n_keep is None else min(int(k[i]), max(int(n_keep), int(nact[i])))
+            n_fill = k_fill - int(nact[i])
+            if n_fill > 0:
+                _fill_null_vectors_z(lib, int(m[i]), int(n[i]), int(k[i]), int(nact[i]), n_fill, bool(transp[i]),
+                                     (bufU, bufU_im), int(u_off[i]), (bufV, bufV_im), int(v_off[i]))
+            lo, hi = int(s_off[i]) + int(nact[i]), int(s_off[i]) + int(k[i])
+            S_h[lo:lo + n_fill] = np.maximum(S_h[lo:lo + n_fill], 1.e-99)
+            S_h[lo + n_fill:hi] = 0.
+        svd_stats['completions'] = svd_stats.get('completions', 0) + 1
+        bufS = backend.to_device(S_h)
+    elif np.any(nact < k):
         # numerically rank-deficient blocks: the kernel left the vectors of the negligible directions on one side
         # zero; complete them to an orthonormal basis (LAPACK returns a complete basis, reference npc:4950)
         n_fill = np.zeros(len(k), dtype=np.int64)
@@ -1545,6 +1596,10 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
         return S
     U._set_blocks(lay_U, bufU)
     VH._set_blocks(lay_V, bufV)
+    if cplx:
+        U_im = Array(U.legs, np.float64, U.qtotal)._set_blocks(lay_U, bufU_im)
+        VH_im = Array(VH.legs, np.float64, VH.qtotal)._set_blocks(lay_V, bufV_im)
+        U, VH = ComplexArray(U, U_im), ComplexArray(VH, VH_im)
     if cutoff is not None:
         keep = S > cutoff
         if not np.any(keep):
@@ -1662,6 +1717,63 @@ def _fill_null_vectors(lib, m, n, k, r, kf, transposed, bufU, u_off, bufV, v_off
         _strided_copy(lib, X, 0, bufU, u_off + r, [kf, m], [m, 1], [1, k])
 
 
+def _fill_null_vectors_z(lib, m, n, k, r, kf, transposed, bufU, u_off, bufV, v_off):
+    """complex counterpart of :func:`_fill_null_vectors` (`bufU`, `bufV` = (real, imaginary) planes): the `r` orthonormal
+    vectors `v_i` (length `p`) of the accumulated side, followed by the `kf` unit vectors of smallest leverage, are the
+    columns of ``M`` (p x (r + kf)); the Householder QR kernel gives ``M = Q R`` with orthonormal columns, the first `r`
+    spanning the `v_i`, so columns ``r .. r+kf-1`` of `Q` are orthonormal and orthogonal to them.  Unlike the
+    Newton-Schulz completion this cannot fail: the reflectors are unitary whatever the conditioning of `M`."""
+    p = m if transposed else n
+    c = r + kf
+    rows = [backend.empty(max(r, 1) * p) for _ in range(2)]     # the r vectors as rows (r x p), both planes
+    if r > 0:
+        for part, buf in enumerate(bufU if transposed else bufV):
+            if transposed:          # columns 0..r-1 of U (m x k)
+                _strided_copy(lib, buf, u_off, rows[part], 0, [r, m], [1, k], [m, 1])
+            else:                   # rows 0..r-1 of VT (k x n)
+                rows[part][:r * n].copy_(buf[v_off:v_off + r * n])
+        lev = backend.empty(p)
+        lev_im = backend.empty(p)
+        lib.col_sqnorms(r, p, p, rows[0], lev)
+        lib.col_sqnorms(r, p, p, rows[1], lev_im)
+        sel = np.sort(np.argsort(backend.to_host(lev) + backend.to_host(lev_im), kind='stable')[:kf]).astype(np.int64)
+    else:
+        sel = np.arange(kf, dtype=np.int64)
+    M = [backend.zeros(p * c) for _ in range(2)]
+    if r > 0:
+        for part in range(2):
+            _strided_copy(lib, rows[part], 0, M[part], 0, [r, p], [p, 1], [1, c])
+    ones = _dev_const('one', lambda: np.ones(1))[1]
+    seg = np.ascontiguousarray(np.stack([np.zeros(kf, np.int64), sel * c + r + np.arange(kf, dtype=np.int64),
+                                         np.ones(kf, np.int64)], axis=1))
+    lib.axpy_segments(len(seg), backend.to_device(seg), 1, 1., ones, M[0])
+    Q = [backend.empty(p * c) for _ in range(2)]
+    R = [backend.empty(c * c) for _ in range(2)]
+    lib.block_qr_z([p], [c], [0], [0], [0], M[0], M[1], Q[0], Q[1], R[0], R[1])
+    for part in range(2):
+        if transposed:              # columns r.. of U <- columns r.. of Q
+            _strided_copy(lib, Q[part], r, bufU[part], u_off + r, [p, kf], [c, 1], [k, 1])
+        else:                       # rows r.. of VT <- columns r.. of Q
+            _strided_copy(lib, Q[part], r, bufV[part], v_off + r * n, [kf, p], [1, c], [p, 1])
+
+
+def _complex_planes(a):
+    """``(layout, buf_re, buf_im)``: the two parts of the ComplexArray `a` on ONE block table.  Each part drops its own
+    zero blocks, so their tables can differ; a block missing in one part is a zero block there."""
+    lr, li = a.re._layout, a.im._layout
+    if lr.same_blocks(li):
+        return lr, a.re._buf, a.im._buf
+    union, seg_re, seg_im = _union_layout(a.legs, lr, li)
+    lib = backend.get_lib()
+    bufs = []
+    for seg, part in ((seg_re, a.re), (seg_im, a.im)):
+        buf = backend.zeros(union.size)
+        if len(seg):
+            lib.axpy_segments(len(seg), backend.to_device(seg), int(seg[:, 2].max()), 1.0, part._buf, buf)
+        bufs.append(buf)
+    return union, bufs[0], bufs[1]
+
+
 qr_stats = {'calls': 0, 'columns': 0, 'replaced': 0}   # diagnostics of the Gram-Schmidt QR
 # 'householder': b200_block_qr_f64, one CTA per block, one launch for all blocks; 'cgs2': Gram-Schmidt on the GEMM /
 # BLAS-1 kernels (one host round trip per column); 'auto' (default): Householder for blocks up to QR_HOUSEHOLDER_MAX rows
@@ -1739,7 +1851,8 @@ def qr(a, mode='reduced', inner_labels=[None, None], cutoff=None, pos_diag_R=Fal
 
     Only ``mode='reduced'`` and ``cutoff=None``.  The diagonal of `R` is positive by construction (Gram-Schmidt, see
     :func:`_block_qr_cgs2`), i.e. the result is the unique decomposition the reference returns for
-    ``pos_diag_R=True`` (for full-rank blocks)."""
+    ``pos_diag_R=True`` (for full-rank blocks).  A :class:`ComplexArray` `a` goes through the complex Householder kernel
+    (``b200_block_qr_z``, every block size); `Q` and `R` are then ComplexArrays, the diagonal of `R` real and >= 0."""
     if a.rank != 2:
         raise ValueError('expect a matrix!')
     if mode != 'reduced':
@@ -1750,7 +1863,11 @@ def qr(a, mode='reduced', inner_labels=[None, None], cutoff=None, pos_diag_R=Fal
     label_Q, label_R = inner_labels
     piped_axes, a = a.as_completely_blocked()
     chinfo = a.chinfo
-    lay = a._layout
+    cplx = isinstance(a, ComplexArray)
+    if cplx:
+        lay, bufA_re, bufA_im = _complex_planes(a)
+    else:
+        lay = a._layout
     a_leg0 = a.legs[0]
     m, n = lay.shapes[:, 0], lay.shapes[:, 1]
     k = np.minimum(m, n)
@@ -1783,19 +1900,31 @@ def qr(a, mode='reduced', inner_labels=[None, None], cutoff=None, pos_diag_R=Fal
         bufQ = backend.zeros(lay_Q.size)
         bufR = backend.zeros(lay_R.size)
         lib = backend.get_lib()
-        small = np.ones(lay.nblocks, bool) if qr_method == 'householder' else \
-            (np.maximum(m, n) <= QR_HOUSEHOLDER_MAX if qr_method == 'auto' else np.zeros(lay.nblocks, bool))
-        if np.any(small):
-            lib.block_qr(m[small], n[small], lay.offsets[small], q_off[small], r_off[small], a._buf, bufQ, bufR)
-        if not np.all(small):
-            for b in np.nonzero(~small)[0]:
-                mb, nb, kb = int(m[b]), int(n[b]), int(k[b])
-                ao = int(lay.offsets[b])
-                _block_qr_cgs2(lib, mb, nb, a._buf[ao:ao + mb * nb], bufQ[int(q_off[b]):int(q_off[b]) + mb * kb],
-                               bufR[int(r_off[b]):int(r_off[b]) + kb * nb])
+        if cplx:         # complex: the Householder kernel for every block size
+            Q_im, R_im = Array(Q.legs, np.float64, Q.qtotal), Array(R.legs, np.float64, R.qtotal)
+            bufQ_im = backend.zeros(lay_Q.size)
+            bufR_im = backend.zeros(lay_R.size)
+            lib.block_qr_z(m, n, lay.offsets, q_off, r_off, bufA_re, bufA_im, bufQ, bufQ_im, bufR, bufR_im)
+            Q_im._set_blocks(lay_Q, bufQ_im)
+            R_im._set_blocks(lay_R, bufR_im)
+        else:
+            small = np.ones(lay.nblocks, bool) if qr_method == 'householder' else \
+                (np.maximum(m, n) <= QR_HOUSEHOLDER_MAX if qr_method == 'auto' else np.zeros(lay.nblocks, bool))
+            if np.any(small):
+                lib.block_qr(m[small], n[small], lay.offsets[small], q_off[small], r_off[small], a._buf, bufQ, bufR)
+            if not np.all(small):
+                for b in np.nonzero(~small)[0]:
+                    mb, nb, kb = int(m[b]), int(n[b]), int(k[b])
+                    ao = int(lay.offsets[b])
+                    _block_qr_cgs2(lib, mb, nb, a._buf[ao:ao + mb * nb], bufQ[int(q_off[b]):int(q_off[b]) + mb * kb],
+                                   bufR[int(r_off[b]):int(r_off[b]) + kb * nb])
         Q._set_blocks(lay_Q, bufQ)
         R._set_blocks(lay_R, bufR)
         qr_stats['calls'] += 1
+    elif cplx:
+        Q_im, R_im = Array(Q.legs, np.float64, Q.qtotal), Array(R.legs, np.float64, R.qtotal)
+    if cplx:
+        Q, R = ComplexArray(Q, Q_im), ComplexArray(R, R_im)
     if 0 in piped_axes:
         Q = Q.split_legs(0)
     if 1 in piped_axes:
@@ -1825,6 +1954,8 @@ def eigh(a, UPLO='L', sort=None):
     Returns ``(W, V)``: eigenvalues (1D host array, ordered like the first leg; within a block ascending or
     as requested by `sort`) and the unitary `V` with legs ``(a.legs[0], a.legs[0].conj() as LegCharge)``.
     Missing diagonal blocks give eigenvalue 0 with unit vectors, exactly like the reference."""
+    if isinstance(a, ComplexArray):
+        raise NotImplementedError('eigh of a complex Hermitian matrix is not implemented (only real symmetric blocks)')
     if a.rank != 2 or a.shape[0] != a.shape[1]:
         raise ValueError('expect a square matrix!')
     a.legs[0].test_contractible(a.legs[1])
@@ -1891,8 +2022,9 @@ def eigh(a, UPLO='L', sort=None):
 
 
 def to_iterable_arrays(array_list):
-    """Flatten nested lists of Arrays (reference npc:2996)."""
-    if isinstance(array_list, Array):
+    """Flatten nested lists of Arrays (reference npc:2996).  An Array (ComplexArray included), a string (an operator name,
+    as in ``MPS.expectation_value('Sz')``) or any other non-iterable is one entry."""
+    if isinstance(array_list, (Array, str)) or not np.iterable(array_list):
         return [array_list]
     return list(itertools.chain.from_iterable(to_iterable_arrays(a) for a in array_list))
 
