@@ -184,7 +184,9 @@ int b200_scale_axis_f64(int64_t n_tasks, const int64_t *task_dev, const int64_t 
 /* Batched Householder QR: block i is A_i (m_i x n_i, row-major at A + a_off[i]); Q_i (m_i x k_i, k = min(m, n)) is
  * written to Q + q_off[i], R_i (k_i x n_i, upper triangular, non-negative diagonal) to R + r_off[i].  One CTA per block,
  * one launch, no host round trip.  replaces the per-block np.linalg.qr of npc.qr (np_conserved.py:4139).  `work` =
- * device scratch of b200_block_qr_worksize bytes.  Used for blocks up to 384 rows / columns (np_conserved.qr_method = 'auto'). */
+ * device scratch of b200_block_qr_worksize bytes.  Used for blocks up to 384 rows / columns (np_conserved.qr_method = 'auto').
+ * Range: every finite block.  Each block is factored as 2^-e A_i, 2^e the power of two of max |a_ij| (exact), and R is
+ * scaled back by 2^e: Q is bit for bit that of 2^-e A_i and R exactly 2^e times its R (rounded once where it is subnormal). */
 int64_t b200_block_qr_worksize(int64_t nblocks, const int64_t *m_host, const int64_t *n_host);
 int b200_block_qr_f64(int64_t nblocks, const int64_t *m_host, const int64_t *n_host, const int64_t *a_off_host,
                       const int64_t *q_off_host, const int64_t *r_off_host, const double *A, double *Q, double *R,
@@ -221,6 +223,13 @@ int b200_col_sqnorms_f64(int64_t rows, int64_t cols, int64_t ld, const double *X
  * orthonormal completion by the caller when it is needed (tenpy_b200.linalg.np_conserved.svd does).
  * nact_host[i] (may be NULL) = number of significant directions (they come first), transposed_host[i] (may be
  * NULL) = 1 if the zero vectors are columns of U_i, 0 if they are rows of VT_i.
+ * Range: every finite block.  The iteration runs on 2^-e A_i, 2^e the power of two of max |a_ij| (exact): U, VT, nact
+ * and transposed are bit for bit those of 2^-e A_i, S is exactly 2^e times its S (rounded once where it is subnormal).
+ * The rotation criteria take square roots separately where a product of Gram entries under- or overflows, and row norms
+ * whose plain sum of squares falls below 2^-900 are summed again rescaled, so rows graded far below the block's largest
+ * entry neither stall the iteration nor lose their norm.  With deflation off (b200_svd_set_deflation(0)), rows whose
+ * squared norm in the scaled block is at most 2^-990 (about 1e-149 max |a_ij|) are left unrotated: their Gram entries
+ * are below the resolution of double precision.  With deflation on they lie far below the threshold anyway.
  * replaces _svd_worker npc:4950 -> svd_robust.svd svd_robust.py:37 (LAPACK gesdd / gesvd). */
 /* switch the deflation of negligible directions in b200_block_svd_f64 on (default) / off; returns the old value */
 int b200_svd_set_deflation(int on);
@@ -254,7 +263,8 @@ int b200_block_svd_f64(int64_t nblocks, const int64_t *m_host, const int64_t *n_
  * One-sided block Jacobi in complex arithmetic (Gram matrix P P^H, complex 2x2 rotations, real FP64 tensor-core products
  * on the planes); no block-size limit.  Rank-deficient blocks: as in the real entry, the vectors of the negligible
  * directions on the non-accumulated side are left ZERO (nact_host / transposed_host say which); the caller completes them
- * (tenpy_b200.linalg.np_conserved.svd does it with b200_block_qr_z).  Never produces NaN for finite input.
+ * (tenpy_b200.linalg.np_conserved.svd does it with b200_block_qr_z).  Never produces NaN for finite input.  Range and
+ * power-of-two scaling of the block: as b200_block_svd_f64 (max over the real and imaginary parts).
  * replaces _svd_worker npc:4950 -> svd_robust.svd (LAPACK zgesdd / zgesvd) for complex blocks. */
 int64_t b200_block_svd_z_worksize(int64_t nblocks, const int64_t *m_host, const int64_t *n_host);
 int b200_block_svd_z(int64_t nblocks, const int64_t *m_host, const int64_t *n_host, const int64_t *a_off_host,
@@ -266,7 +276,8 @@ int b200_block_svd_z(int64_t nblocks, const int64_t *m_host, const int64_t *n_ho
  * sharing one offset table; Q_i (m_i x k_i) with orthonormal columns, R_i (k_i x n_i) upper triangular with a real
  * non-negative diagonal.  One CTA per block, one launch, every block size (cost O(m n k) on one SM: meant for the
  * canonical-form path, not for large dense blocks).  replaces the per-block np.linalg.qr of npc.qr (np_conserved.py:4139)
- * for complex blocks.  `work` = device scratch of b200_block_qr_z_worksize bytes. */
+ * for complex blocks.  `work` = device scratch of b200_block_qr_z_worksize bytes.  Range and power-of-two scaling of the
+ * block: as b200_block_qr_f64 (max over the real and imaginary parts). */
 int64_t b200_block_qr_z_worksize(int64_t nblocks, const int64_t *m_host, const int64_t *n_host);
 int b200_block_qr_z(int64_t nblocks, const int64_t *m_host, const int64_t *n_host, const int64_t *a_off_host,
                     const int64_t *q_off_host, const int64_t *r_off_host, const double *A_re, const double *A_im,
@@ -275,6 +286,8 @@ int b200_block_qr_z(int64_t nblocks, const int64_t *m_host, const int64_t *n_hos
 
 /* Batched symmetric eigen-decomposition of nblocks row-major symmetric matrices A_i (n[i] x n[i]):
  * A_i = V_i diag(W_i) V_i^T, W_i ascending, eigenvectors in the COLUMNS of V_i (row-major n x n).
+ * Range: every finite block.  The iteration runs on 2^-e A_i, 2^e the power of two of max |a_ij| (exact): V is bit for
+ * bit that of 2^-e A_i, W exactly 2^e times its W (rounded once where it is subnormal).  Accuracy |A_i|_F-normwise.
  * replaces _eig_worker npc:5041 (np.linalg.eigh, LAPACK syevd). */
 int64_t b200_block_eigh_worksize(int64_t nblocks, const int64_t *n_host);
 int b200_block_eigh_f64(int64_t nblocks, const int64_t *n_host, const int64_t *a_off_host,

@@ -11,9 +11,14 @@
 // cross-thread quantity per Householder step is the squared norm of the pivot column below the diagonal, summed in a
 // fixed order from per-thread partials (deterministic).  Every phase is a plain function of (tid, nthreads, pointers):
 // the CUDA kernel runs it per thread between __syncthreads(), tests/csrc/block_qr_host.cpp runs it for tid = 0..T-1.
+//
+// The factorisation runs on 2^-e A (scaling.cuh: the largest entry in [1, 2)), so that the column norms neither under- nor
+// overflow for any finite block; R is scaled back exactly on output, Q is the same bit for bit.
 #pragma once
 #include <cmath>
 #include <cstdint>
+
+#include "scaling.cuh"
 
 #if defined(__CUDACC__)
 #define BQ_HD __host__ __device__ __forceinline__
@@ -23,6 +28,33 @@
 
 namespace b200 {
 namespace bqr {
+
+// PHASE 0: partial[tid] = max |X[e]| over this thread's entries of the len entries of X (and Xi, if not NULL)
+BQ_HD void absmax_partial(int tid, int T, const double *X, const double *Xi, int64_t len, double *partial) {
+    double a = 0.0;
+    for (int64_t e = tid; e < len; e += T) {
+        a = fmax(a, fabs(X[e]));
+        if (Xi) a = fmax(a, fabs(Xi[e]));
+    }
+    partial[tid] = a;
+}
+
+// PHASE 0 (every thread, after the barrier): the block scale pow2_scale(max |A|) from the partials
+BQ_HD double block_scale(int T, const double *partial) {
+    double a = 0.0;
+    for (int t = 0; t < T; ++t) a = fmax(a, partial[t]);
+    return b200::pow2_scale(a);
+}
+
+// PHASE 0 (after block_scale): A[e] = A_in[e] * scale, the working copy the factorisation runs on
+BQ_HD void scale_in(int tid, int T, const double *A_in, double *A, int64_t len, double scale) {
+    for (int64_t e = tid; e < len; e += T) A[e] = A_in[e] * scale;
+}
+
+// LAST PHASE: R_out = the first k rows of A times rscale = 1 / scale (exact: a power of two)
+BQ_HD void store_r(int tid, int T, const double *A, double *R_out, int k, int n, double rscale) {
+    for (int64_t e = tid; e < (int64_t)k * n; e += T) R_out[e] = A[e] * rscale;
+}
 
 // PHASE 1: partial[tid] = sum over rows r > j (strided by threads) of A[r][j]^2
 BQ_HD void col_partial(int tid, int T, const double *A, int m, int n, int j, double *partial) {

@@ -33,7 +33,10 @@ __global__ void __launch_bounds__(QR_THREADS) block_qr_kernel(const QrBlk *__res
     double *tau = V + (int64_t)m * k;                 // k
     double *sign = tau + k;                           // k
     double *Q = Q_out + b.q_off;
-    for (int64_t e = tid; e < (int64_t)m * n; e += T) A[e] = A_in[b.a_off + e];
+    bqr::absmax_partial(tid, T, A_in + b.a_off, nullptr, (int64_t)m * n, partial);
+    __syncthreads();
+    const double scale = bqr::block_scale(T, partial), rscale = 1.0 / scale;   // exact: powers of two
+    bqr::scale_in(tid, T, A_in + b.a_off, A, (int64_t)m * n, scale);
     __syncthreads();
     for (int j = 0; j < k; ++j) {
         bqr::col_partial(tid, T, A, m, n, j, partial);
@@ -58,7 +61,7 @@ __global__ void __launch_bounds__(QR_THREADS) block_qr_kernel(const QrBlk *__res
     __syncthreads();
     bqr::flip_signs(tid, T, A, Q, m, n, k, sign);
     __syncthreads();
-    for (int64_t e = tid; e < (int64_t)k * n; e += T) R_out[b.r_off + e] = A[e];
+    bqr::store_r(tid, T, A, R_out + b.r_off, k, n, rscale);
 }
 
 static inline int64_t qr_work_elems(int64_t m, int64_t n) {
@@ -86,9 +89,12 @@ __global__ void __launch_bounds__(QR_THREADS) block_qr_z_kernel(const QrBlk *__r
     double *Vr = Ai + mn, *Vi = Vr + mk;              // m x k reflectors
     double *taur = Vi + mk, *taui = taur + k;         // k
     double *Qr = Qr_out + b.q_off, *Qi = Qi_out + b.q_off;
+    bqr::absmax_partial(tid, T, Ar_in + b.a_off, Ai_in + b.a_off, mn, partial);
+    __syncthreads();
+    const double scale = bqr::block_scale(T, partial), rscale = 1.0 / scale;   // block_qr_core.cuh: exact
     for (int64_t e = tid; e < mn; e += T) {
-        Ar[e] = Ar_in[b.a_off + e];
-        Ai[e] = Ai_in[b.a_off + e];
+        Ar[e] = Ar_in[b.a_off + e] * scale;
+        Ai[e] = Ai_in[b.a_off + e] * scale;
     }
     __syncthreads();
     for (int j = 0; j < k; ++j) {
@@ -190,8 +196,8 @@ __global__ void __launch_bounds__(QR_THREADS) block_qr_z_kernel(const QrBlk *__r
     for (int64_t e = tid; e < (int64_t)k * n; e += T) {
         const int i = (int)(e / n), c = (int)(e % n);
         const double sg = Ar[(int64_t)i * n + i] < 0.0 ? -1.0 : 1.0;
-        Rr_out[b.r_off + e] = c < i ? 0.0 : sg * Ar[e];
-        Ri_out[b.r_off + e] = c < i ? 0.0 : sg * Ai[e];
+        Rr_out[b.r_off + e] = c < i ? 0.0 : sg * Ar[e] * rscale;
+        Ri_out[b.r_off + e] = c < i ? 0.0 : sg * Ai[e] * rscale;
     }
     for (int64_t e = tid; e < mk; e += T) {
         const int i = (int)(e % k);

@@ -25,6 +25,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "scaling.cuh"
 
 namespace b200 {
 
@@ -55,11 +56,24 @@ struct JMat {
     double defl;                           // deflation threshold: rows with norm <= defl are negligible
     double shift;                          // eigh: diagonal shift
     int64_t yi_off, wi_off;                // complex SVD: imaginary parts of Y and W (planar; y_off / w_off = real parts)
-    double scale;                          // complex SVD: Y = scale * A (a power of two, |scale A|_F ~ 1), S = norms / scale
+    double scale;                          // Y = scale * A, scale = pow2_scale(max |a_ij|) (exact); S, W = norms / scale
     int32_t cplx, pad_;                    // 1: complex matrix (b200_block_svd_z)
+    double amax;                           // max |a_ij| (jacobi_amax_kernel; 0 before it runs)
 };
 
 constexpr int jacobi_smem_bytes() { return 2 * JP * JLDP * (int)sizeof(double); }   // two panel chunks
+
+// Gram diagonals at or below J_GRAM_MIN (Y is the scaled block, max |y| in [1, 2)) are lost in the absolute rounding of
+// subnormal products (~p 2^-1075 per entry): such rows cannot be resolved and are inert, like deflated ones.  Far below
+// any deflation threshold, so this only decides anything with deflation off, for rows graded below ~1e-149.
+constexpr double J_GRAM_MIN = 0x1p-990;
+__device__ __forceinline__ bool j_normal(double x) { return x >= 2.2250738585072014e-308 && x <= 1.7976931348623157e308; }
+// sqrt(a b) for a, b >= 0 without under- or overflow of the product.  Where the product is normal this is the plain
+// sqrt(a * b), so every decision on normal-range data is the one it always was.
+__device__ __forceinline__ double j_sqrt_prod(double a, double b) {
+    const double d = a * b;
+    return j_normal(d) ? sqrt(d) : sqrt(a) * sqrt(b);
+}
 
 __device__ __forceinline__ void j_load_chunk(double *sP, const double *base, int ld, const int *prow, int col0,
                                              int tid) {
@@ -246,16 +260,15 @@ __global__ void __launch_bounds__(JTHREADS)
     __syncthreads();
 
     // ---- convergence measure of this pair ----
-    const double defl2 = mt.defl * mt.defl;
+    const double defl2 = fmax(mt.defl * mt.defl, J_GRAM_MIN);
     double offmax = 0.0;
     for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
         int r = idx / JP, c = idx % JP;
         if (r < c) {
             const double drr = sG[r * JLDG + r], dcc = sG[c * JLDG + c];
-            double d = drr * dcc;
             double o = fabs(sG[r * JLDG + c]);
             if (drr > defl2 && dcc > defl2) {   // negligible (deflated) rows are inert
-                double v = o / sqrt(d);
+                double v = o / j_sqrt_prod(drr, dcc);
                 offmax = fmax(offmax, v);
             }
         }
@@ -296,11 +309,13 @@ __global__ void __launch_bounds__(JTHREADS)
                 int p = a < b ? a : b, q = a < b ? b : a;
                 double gpp = sG[p * JLDG + p], gqq = sG[q * JLDG + q], gpq = sG[p * JLDG + q];
                 double c = 1.0, s = 0.0;
-                double lim = tol_in * sqrt(fabs(gpp * gqq));
+                double lim = tol_in * j_sqrt_prod(fabs(gpp), fabs(gqq));
                 if (fabs(gpq) > lim && gpp > defl2 && gqq > defl2) {
-                    // t = tan(theta) of the Jacobi rotation: one sqrt, one division, one rsqrt
+                    // t = tan(theta) of the Jacobi rotation: one sqrt, one division, one rsqrt (hypot where aa^2 + bb^2
+                    // is not a normal number)
                     const double aa = gqq - gpp, bb = 2.0 * gpq;
-                    const double hh = sqrt(aa * aa + bb * bb);
+                    const double h2 = aa * aa + bb * bb;
+                    const double hh = j_normal(h2) ? sqrt(h2) : hypot(aa, bb);
                     const double tt = (aa >= 0.0) ? bb / (aa + hh) : bb / (aa - hh);
                     c = rsqrt(1.0 + tt * tt);
                     s = tt * c;
@@ -337,12 +352,12 @@ __global__ void __launch_bounds__(JTHREADS)
         if (!__syncthreads_or(any)) break;
     }
     // order the new rows by descending eigenvalue (norm^2): helps the outer convergence (de Rijk)
-    // rank[i] = number of entries with larger diagonal (ties by index)
+    // rank[i] = number of entries with larger diagonal (ties by index); the key is clamped at 0 (see zjacobi_eig_kernel)
     if (tid < JP) {
-        double di = sG[tid * JLDG + tid];
+        double di = fmax(sG[tid * JLDG + tid], 0.0);
         int rk = 0;
         for (int k = 0; k < JP; ++k) {
-            double dk = sG[k * JLDG + k];
+            double dk = fmax(sG[k * JLDG + k], 0.0);
             if (dk > di || (dk == di && k < tid)) ++rk;
         }
         // store rank in sG's unused padding column
@@ -452,7 +467,7 @@ __device__ __forceinline__ void jacobi_eig_v3_body(const JMat *__restrict__ mats
     if (tid == 0) s_any = 0;
     __syncthreads();
     // ---- convergence measure of this pair (as version 1) ----
-    const double defl2 = mt.defl * mt.defl;
+    const double defl2 = fmax(mt.defl * mt.defl, J_GRAM_MIN);
     double offmax = 0.0;
     {
         const double dl = sA[lane * JLDG + lane];
@@ -460,7 +475,7 @@ __device__ __forceinline__ void jacobi_eig_v3_body(const JMat *__restrict__ mats
         for (int i = 0; i < 4; ++i) {
             const int c = 4 * warp + i;
             const double dc = sA[c * JLDG + c];
-            if (lane < c && dl > defl2 && dc > defl2) offmax = fmax(offmax, fabs(g[i]) / sqrt(dl * dc));
+            if (lane < c && dl > defl2 && dc > defl2) offmax = fmax(offmax, fabs(g[i]) / j_sqrt_prod(dl, dc));
         }
     }
     offmax = warp_max(offmax);
@@ -491,7 +506,10 @@ __device__ __forceinline__ void jacobi_eig_v3_body(const JMat *__restrict__ mats
             const int p = is_p ? lane : partner, q = is_p ? partner : lane;
             const double gpp = sA[p * JLDG + p], gqq = sA[q * JLDG + q], gpq = sA[p * JLDG + q];
             double c = 1.0, sn = 0.0;
-            if (gpq * gpq > (tol_in * tol_in) * fabs(gpp * gqq) && gpp > defl2 && gqq > defl2) {
+            // |g_pq| > tol_in sqrt(g_pp g_qq), squared; with square roots taken separately where a product is not normal
+            const double g2 = gpq * gpq, rhs = (tol_in * tol_in) * fabs(gpp * gqq);
+            const bool off = (j_normal(g2) && j_normal(rhs)) ? g2 > rhs : fabs(gpq) > tol_in * j_sqrt_prod(fabs(gpp), fabs(gqq));
+            if (off && gpp > defl2 && gqq > defl2) {
                 jeig3_rotation(gpp, gqq, gpq, c, sn);
                 if (warp == 0) s_any = 1;     // benign race: every writer stores 1
             }
@@ -527,12 +545,13 @@ __device__ __forceinline__ void jacobi_eig_v3_body(const JMat *__restrict__ mats
         if (tid == 0) s_any = 0;
         __syncthreads();
     }
-    // order the new rows by descending eigenvalue (norm^2): rank[i] = number of entries with larger diagonal (ties by index)
+    // order the new rows by descending eigenvalue (norm^2): rank[i] = number of entries with larger diagonal (ties by index);
+    // the key is clamped at 0, as in zjacobi_eig_kernel: a rank-deficient block must not lose a row to a padding row
     if (tid < JP) {
-        const double di = sA[tid * JLDG + tid];
+        const double di = fmax(sA[tid * JLDG + tid], 0.0);
         int rk = 0;
         for (int k = 0; k < JP; ++k) {
-            const double dk = sA[k * JLDG + k];
+            const double dk = fmax(sA[k * JLDG + k], 0.0);
             if (dk > di || (dk == di && k < tid)) ++rk;
         }
         s_rank[tid] = rk;
@@ -716,7 +735,7 @@ __global__ void __launch_bounds__(JTHREADS)
 
     // ---- convergence measure of this pair: max |g_rc| / sqrt(g_rr g_cc) over the non-negligible rows ----
     // (square roots taken separately and hypot below: g_rr g_cc over- or underflows for blocks scaled near 1e+-150)
-    const double defl2 = mt.defl * mt.defl;
+    const double defl2 = fmax(mt.defl * mt.defl, J_GRAM_MIN);
     double offmax = 0.0;
     for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
         const int r = idx / JP, c = idx % JP;
@@ -917,32 +936,64 @@ __global__ void __launch_bounds__(JTHREADS)
 }
 
 // ---- init / finalize kernels ---------------------------------------------------------------------
-// squared row norms (first m entries) and column norms (next n entries) of every A: grid (m + n, nmat).
+// mats[b].amax = max |a_ij| over the m x n entries of A (and Ai); amax must be 0 on entry.  grid (chunks, nmat), 256
+// threads.  Non-negative doubles order like their bit patterns, so the CTA maxima combine exactly by an integer atomicMax.
+// The block scale pow2_scale(amax) (scaling.cuh) follows; every later norm and Gram entry is formed on scale * A
+__global__ void __launch_bounds__(256) jacobi_amax_kernel(JMat *__restrict__ mats, const double *__restrict__ A,
+                                                          const double *__restrict__ Ai) {
+    __shared__ double red[32];
+    JMat *mt = mats + blockIdx.y;
+    const int64_t mn = (int64_t)mt->m * mt->n;
+    const int64_t a0 = mt->a_off;
+    double amax = 0.0;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < mn; e += (int64_t)gridDim.x * blockDim.x) {
+        amax = fmax(amax, fabs(A[a0 + e]));
+        if (Ai) amax = fmax(amax, fabs(Ai[a0 + e]));
+    }
+    amax = warp_max(amax);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = amax;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) amax = fmax(amax, red[w]);
+        if (amax > 0.0)
+            atomicMax(reinterpret_cast<unsigned long long *>(&mt->amax), (unsigned long long)__double_as_longlong(amax));
+    }
+}
+
+static void launch_amax(const std::vector<JMat> &mats, JMat *d_mats, const double *A, const double *Ai, cudaStream_t st) {
+    int64_t max_elems = 0;
+    for (auto &mt : mats) max_elems = std::max<int64_t>(max_elems, (int64_t)mt.m * mt.n);
+    const int64_t gx = std::min<int64_t>(std::max<int64_t>(1, (max_elems + 4095) / 4096), 1024);
+    jacobi_amax_kernel<<<dim3((unsigned)gx, (unsigned)mats.size()), 256, 0, st>>>(d_mats, A, Ai);
+}
+
+// squared row norms (first m entries) and column norms (next n entries) of every scale * A: grid (m + n, nmat).
 // Ai (complex input, else NULL): imaginary part, |a|^2 = re^2 + im^2
 __global__ void __launch_bounds__(128) svd_prep_kernel(double *__restrict__ work, const JMat *__restrict__ mats,
                                                        const double *__restrict__ A, const double *__restrict__ Ai) {
     __shared__ double red[32];
-    const JMat mt = mats[blockIdx.y];
+    JMat mt = mats[blockIdx.y];
     const int v = blockIdx.x;
     if (v >= mt.m + mt.n) return;
+    mt.scale = pow2_scale(mt.amax);   // (the host stores the same value in mats before svd_init_kernel)
     const double *a = A + mt.a_off;
     double s = 0.0;
     if (v < mt.m) {
         for (int c = threadIdx.x; c < mt.n; c += blockDim.x) {
-            double x = a[(int64_t)v * mt.n + c];
+            double x = a[(int64_t)v * mt.n + c] * mt.scale;
             s = fma(x, x, s);
             if (Ai) {
-                x = Ai[mt.a_off + (int64_t)v * mt.n + c];
+                x = Ai[mt.a_off + (int64_t)v * mt.n + c] * mt.scale;
                 s = fma(x, x, s);
             }
         }
     } else {
         const int c = v - mt.m;
         for (int r = threadIdx.x; r < mt.m; r += blockDim.x) {
-            double x = a[(int64_t)r * mt.n + c];
+            double x = a[(int64_t)r * mt.n + c] * mt.scale;
             s = fma(x, x, s);
             if (Ai) {
-                x = Ai[mt.a_off + (int64_t)r * mt.n + c];
+                x = Ai[mt.a_off + (int64_t)r * mt.n + c] * mt.scale;
                 s = fma(x, x, s);
             }
         }
@@ -951,7 +1002,7 @@ __global__ void __launch_bounds__(128) svd_prep_kernel(double *__restrict__ work
     if (threadIdx.x == 0) work[mt.prep_off + v] = s;
 }
 
-// SVD init: Y[r] = vector perm[r] of A (rows of A, or columns if transposed -- not conjugated), zero padded;
+// SVD init: Y[r] = vector perm[r] of scale * A (rows of A, or columns if transposed -- not conjugated), zero padded;
 // W = permutation.  Ai (complex input, else NULL): imaginary part into Yi (Wi stays zero).  grid (chunks, nmat)
 __global__ void __launch_bounds__(256) svd_init_kernel(double *__restrict__ work, const JMat *__restrict__ mats,
                                                        const int *__restrict__ perm, const double *__restrict__ A,
@@ -967,27 +1018,31 @@ __global__ void __launch_bounds__(256) svd_init_kernel(double *__restrict__ work
         int r = (int)(e / mt.p), c = (int)(e % mt.p);
         int src = pm[r];
         const int64_t ia = mt.transposed ? (int64_t)c * mt.n + src : (int64_t)src * mt.n + c;
-        if (Ai) {
-            Y[(int64_t)r * mt.ldy + c] = a[ia] * mt.scale;
-            work[mt.yi_off + (int64_t)r * mt.ldy + c] = Ai[mt.a_off + ia] * mt.scale;
-        } else {
-            Y[(int64_t)r * mt.ldy + c] = a[ia];
-        }
+        Y[(int64_t)r * mt.ldy + c] = a[ia] * mt.scale;
+        if (Ai) work[mt.yi_off + (int64_t)r * mt.ldy + c] = Ai[mt.a_off + ia] * mt.scale;
     }
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < mt.qp; e += stride)
         W[e * mt.ldw + (e < mt.q ? pm[e] : e)] = 1.0;
 }
 
-// eigh init: Y = A + shift*I.  shift[mat] was computed by eigh_shift_kernel.
+// eigh init: Y = scale * A + shift*I.  scale[mat] and shift[mat] are set by eigh_shift_kernel (after jacobi_amax_kernel).
 __global__ void __launch_bounds__(256) eigh_shift_kernel(JMat *__restrict__ mats, const double *__restrict__ A) {
     __shared__ double red[32];
     JMat *mt = mats + blockIdx.x;
     const double *a = A + mt->a_off;
+    const double scale = pow2_scale(mt->amax);
     const int64_t nn = (int64_t)mt->n * mt->n;
     double s = 0.0;
-    for (int64_t e = threadIdx.x; e < nn; e += blockDim.x) s = fma(a[e], a[e], s);
+    for (int64_t e = threadIdx.x; e < nn; e += blockDim.x) {
+        const double x = a[e] * scale;
+        s = fma(x, x, s);
+    }
     s = block_sum(s, red);
-    if (threadIdx.x == 0) mt->shift = 1.0625 * sqrt(s) + 1e-300;
+    // (no absolute term: the scaled block has max |a| in [1, 2), and a zero block needs no shift -- W = 0 exactly)
+    if (threadIdx.x == 0) {
+        mt->scale = scale;
+        mt->shift = 1.0625 * sqrt(s);
+    }
 }
 
 __global__ void __launch_bounds__(256) eigh_init_kernel(double *__restrict__ work, const JMat *__restrict__ mats,
@@ -1001,7 +1056,7 @@ __global__ void __launch_bounds__(256) eigh_init_kernel(double *__restrict__ wor
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < ny; e += stride) {
         int r = (int)(e / mt.p), c = (int)(e % mt.p);
         // symmetrise (use both triangles) like a Hermitian solver would see one triangle
-        double v = 0.5 * (a[(int64_t)r * mt.n + c] + a[(int64_t)c * mt.n + r]);
+        double v = 0.5 * (a[(int64_t)r * mt.n + c] * mt.scale + a[(int64_t)c * mt.n + r] * mt.scale);
         if (r == c) v += mt.shift;
         Y[(int64_t)r * mt.ldy + c] = v;
     }
@@ -1009,21 +1064,54 @@ __global__ void __launch_bounds__(256) eigh_init_kernel(double *__restrict__ wor
         W[e * mt.ldw + e] = 1.0;
 }
 
-// row norms of Y: grid (max_q, nmat), 128 threads
+// row norms of Y: grid (max_q, nmat), 128 threads.  A row whose sum of squares is below 2^-900 (squares may have
+// underflowed: rows graded far below the block's largest entry) is summed again scaled by the power of two of its largest
+// entry; every other row gets the plain sum, as it always did.
 __global__ void __launch_bounds__(128) jacobi_norms_kernel(double *__restrict__ work, const JMat *__restrict__ mats) {
     __shared__ double red[32];
+    __shared__ double s_bc;
     const JMat mt = mats[blockIdx.y];
     const int r = blockIdx.x;
     if (r >= mt.q) return;
     const double *y = work + mt.y_off + (int64_t)r * mt.ldy;
+    const double *yi = work + mt.yi_off + (int64_t)r * mt.ldy;
     double s = 0.0;
     for (int c = threadIdx.x; c < mt.p; c += blockDim.x) s = fma(y[c], y[c], s);
-    if (mt.cplx) {
-        const double *yi = work + mt.yi_off + (int64_t)r * mt.ldy;
+    if (mt.cplx)
         for (int c = threadIdx.x; c < mt.p; c += blockDim.x) s = fma(yi[c], yi[c], s);
-    }
     s = block_sum(s, red);
-    if (threadIdx.x == 0) work[mt.snorm_off + r] = sqrt(s);
+    if (threadIdx.x == 0) s_bc = s;
+    __syncthreads();
+    s = s_bc;
+    if (s >= 0x1p-900 || s != s) {
+        if (threadIdx.x == 0) work[mt.snorm_off + r] = sqrt(s);
+        return;
+    }
+    double mx = 0.0;
+    for (int c = threadIdx.x; c < mt.p; c += blockDim.x) {
+        mx = fmax(mx, fabs(y[c]));
+        if (mt.cplx) mx = fmax(mx, fabs(yi[c]));
+    }
+    mx = warp_max(mx);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) mx = fmax(mx, red[w]);
+        s_bc = pow2_scale(mx);
+    }
+    __syncthreads();
+    const double sc = s_bc;
+    double t = 0.0;
+    for (int c = threadIdx.x; c < mt.p; c += blockDim.x) {
+        double x = y[c] * sc;
+        t = fma(x, x, t);
+        if (mt.cplx) {
+            x = yi[c] * sc;
+            t = fma(x, x, t);
+        }
+    }
+    t = block_sum(t, red);
+    if (threadIdx.x == 0) work[mt.snorm_off + r] = sqrt(t) / sc;
 }
 
 // After a sweep, on the device: active-set bookkeeping of every matrix that is still iterating (one CTA per matrix).
@@ -1109,7 +1197,7 @@ __global__ void __launch_bounds__(128)
     const double inv = (s > mt.defl && s > 0.0) ? 1.0 / s : 0.0;   // negligible direction: filled by the caller
     const double *y = work + mt.y_off + (int64_t)src * mt.ldy;
     const double *w = work + mt.w_off + (int64_t)src * mt.ldw;
-    if (threadIdx.x == 0) S[mt.s_off + r] = s;
+    if (threadIdx.x == 0) S[mt.s_off + r] = s / mt.scale;     // exact: scale is a power of two
     double *u = U + mt.u_off;
     double *vt = VT + mt.vt_off;
     if (mt.transposed) {  // Y rows: length m -> U[:, r];  W rows: length n -> VT[r, :]
@@ -1159,7 +1247,7 @@ __global__ void __launch_bounds__(128)
     }
 }
 
-// eigh finalize: eigenvalue r (ascending) = norm[perm[r]] - shift; V[:, r] = W[perm[r], :]
+// eigh finalize: eigenvalue r (ascending) = (norm[perm[r]] - shift) / scale; V[:, r] = W[perm[r], :]
 __global__ void __launch_bounds__(128)
     eigh_finalize_kernel(const double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ perm,
                          double *__restrict__ Wout, double *__restrict__ V) {
@@ -1169,7 +1257,7 @@ __global__ void __launch_bounds__(128)
     if (r >= n) return;
     const int src = perm[mt.perm_off + r];
     const double *w = work + mt.w_off + (int64_t)src * mt.ldw;
-    if (threadIdx.x == 0) Wout[mt.s_off + r] = work[mt.snorm_off + src] - mt.shift;
+    if (threadIdx.x == 0) Wout[mt.s_off + r] = (work[mt.snorm_off + src] - mt.shift) / mt.scale;
     double *v = V + mt.vt_off;
     for (int i = threadIdx.x; i < n; i += blockDim.x) v[(int64_t)i * n + r] = w[i];
 }
@@ -1575,15 +1663,22 @@ static int block_svd_impl(int64_t nblocks, const int64_t *m, const int64_t *n, c
     {
         // orientation + pre-sort: orthogonalise the side whose Gram matrix is closer to diagonal (for square
         // blocks), vectors ordered by descending norm (de Rijk); both from one pass over A.
+        // Both, and the whole iteration, work on scale * A (jacobi_amax_kernel), so that no sum of squares over- or
+        // underflows for any finite block; the threshold `defl` is in the same units.
         int max_mn = 0;
         for (auto &mt : L.mats) max_mn = std::max(max_mn, mt.m + mt.n);
+        launch_amax(L.mats, d_mats, A, Ai, st);
+        B200_CHECK_LAUNCH();
         svd_prep_kernel<<<dim3((unsigned)max_mn, (unsigned)nmat), 128, 0, st>>>(wf, d_mats, A, Ai);
         B200_CHECK_LAUNCH();
+        B200_CUDA_CHECK(cudaMemcpyAsync(L.mats.data(), d_mats, (size_t)nmat * sizeof(JMat), cudaMemcpyDeviceToHost, st));
+        B200_CUDA_CHECK(cudaStreamSynchronize(st));   // L.mats (amax) is read below
         std::vector<int> perm0((size_t)L.perm_elems + 1, 0);
         std::vector<double> nr;
         bool changed = false;
         for (int i = 0; i < nmat; ++i) {
             JMat &mt = L.mats[(size_t)i];
+            mt.scale = pow2_scale(mt.amax);
             nr.resize((size_t)mt.m + mt.n);
             B200_CUDA_CHECK(cudaMemcpyAsync(nr.data(), wf + mt.prep_off, nr.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
             B200_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -1621,13 +1716,6 @@ static int block_svd_impl(int64_t nblocks, const int64_t *m, const int64_t *n, c
                 if (nb_act > mt.nb) nb_act = mt.nb;
                 mt.n_act = n_act;
                 mt.nb_act = nb_act;
-                changed = true;
-            }
-            // complex: iterate on Y = 2^-e A with |Y|_F ~ 1 (exact).  At |A| ~ 1e-150 the converged off-diagonal Gram
-            // entries would be subnormal (the iteration stops early); at 1e+150 large blocks overflow.  The threshold follows.
-            if (cplx && fro2 > 0.0 && std::isfinite(fro2)) {
-                mt.scale = std::ldexp(1.0, -std::ilogb(std::sqrt(fro2)));
-                if (mt.defl > 0.0) mt.defl *= mt.scale;
                 changed = true;
             }
         }
@@ -1729,6 +1817,8 @@ extern "C" int b200_block_eigh_f64(int64_t nblocks, const int64_t *n, const int6
     B200_CUDA_CHECK(cudaMemcpyAsync(work + L.off_cta, L.cta_mat.data(), L.cta_mat.size() * 4, cudaMemcpyHostToDevice, st));
     JMat *d_mats = reinterpret_cast<JMat *>(work + L.off_mats);
     double *wf = reinterpret_cast<double *>(work);
+    launch_amax(L.mats, d_mats, A, nullptr, st);
+    B200_CHECK_LAUNCH();
     eigh_shift_kernel<<<nmat, 256, 0, st>>>(d_mats, A);
     B200_CHECK_LAUNCH();
     {

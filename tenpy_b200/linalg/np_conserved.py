@@ -1550,7 +1550,7 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
                 _fill_null_vectors_z(lib, int(m[i]), int(n[i]), int(k[i]), int(nact[i]), n_fill, bool(transp[i]),
                                      (bufU, bufU_im), int(u_off[i]), (bufV, bufV_im), int(v_off[i]))
             lo, hi = int(s_off[i]) + int(nact[i]), int(s_off[i]) + int(k[i])
-            S_h[lo:lo + n_fill] = np.maximum(S_h[lo:lo + n_fill], 1.e-99)
+            S_h[lo:lo + n_fill] = np.maximum(S_h[lo:lo + n_fill], _completion_floor(S_h[int(s_off[i]):lo]))
             S_h[lo + n_fill:hi] = 0.
         svd_stats['completions'] = svd_stats.get('completions', 0) + 1
         bufS = backend.to_device(S_h)
@@ -1584,7 +1584,7 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
             for i in np.nonzero(nact < k)[0]:
                 lo, hi = int(s_off[i]) + int(nact[i]), int(s_off[i]) + int(k[i])
                 mid = lo + int(n_fill[i])
-                S_h[lo:mid] = np.maximum(S_h[lo:mid], 1.e-99)
+                S_h[lo:mid] = np.maximum(S_h[lo:mid], _completion_floor(S_h[int(s_off[i]):lo]))
                 S_h[mid:hi] = 0.
             bufS = backend.to_device(S_h)
     S = backend.to_host(bufS)
@@ -1618,6 +1618,17 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
 
 class _CompletionFailed(Exception):
     pass
+
+
+def _completion_floor(S_genuine):
+    """lower bound of the singular value of a completed (negligible) direction of a block whose genuine singular values
+    are `S_genuine` (all > 0: they exceed the deflation threshold): 1e-99, but at most eps times the smallest genuine one
+    (and never below the smallest positive double, nor above the smallest genuine one), so that a truncation keeps the
+    genuine directions of a block first at any scale of the block, U S VH stays A to eps, and the bound stays > 0."""
+    if not len(S_genuine):
+        return 1.e-99
+    smin = float(np.min(S_genuine))
+    return min(1.e-99, smin, max(smin * np.finfo(np.float64).eps, 5e-324))
 
 
 _SMALL_DEV_CACHE = {}     # small constant device arrays (copy records, index lists, the scalar 1.) by content
@@ -1782,6 +1793,28 @@ qr_method = 'auto'
 QR_HOUSEHOLDER_MAX = 384
 
 
+_SQ_SAFE = (2.**-900, 2.**900)     # squared norms in this range leave the Gram-Schmidt sums far from over- and underflow
+
+
+def _rescale_column(lib, m, v, sq, scratch, out):
+    """Norm of the column `v` (device, length `m`, squared norm `sq`) after scaling it in place by powers of two
+    (exact) until its squared norm lies in `_SQ_SAFE`; a column already in range is left untouched, a zero column stays
+    zero.  Gram-Schmidt is invariant under column scaling (``A D = Q (R D)``), and R is formed from the unscaled A."""
+    for _ in range(4):
+        if _SQ_SAFE[0] <= sq <= _SQ_SAFE[1] or not sq == sq:
+            break
+        if sq == 0.:
+            e = 600
+        elif sq == np.inf:
+            e = -600
+        else:
+            e = -(int(np.frexp(sq)[1]) // 2)
+        lib.scal(m, 2.**e, v)
+        lib.dot(m, v, v, scratch, out)
+        sq = float(backend.read_scalar(out))
+    return float(np.sqrt(max(sq, 0.)))
+
+
 def _block_qr_cgs2(lib, m, n, A, Q, R):
     """``A (m x n) = Q (m x k) R (k x n)``, ``k = min(m, n)``, on device buffers (row-major views): classical
     Gram-Schmidt with re-orthogonalisation ("twice is enough"), column by column, built from the existing kernels --
@@ -1799,7 +1832,7 @@ def _block_qr_cgs2(lib, m, n, A, Q, R):
     _strided_copy(lib, A, 0, T, 0, [n, m], [1, n], [m, 1])
     cn = backend.empty(n)
     lib.col_sqnorms(m, n, n, A, cn)
-    col_norm = np.sqrt(backend.to_host(cn))
+    col_sq = backend.to_host(cn)
     Qt = backend.zeros(k * m)
     w = backend.empty(max(k, 1))
     tmp = backend.empty(m)
@@ -1807,6 +1840,7 @@ def _block_qr_cgs2(lib, m, n, A, Q, R):
     next_unit = 0
     for j in range(k):
         v = T[j * m:(j + 1) * m].clone()
+        col_norm = _rescale_column(lib, m, v, float(col_sq[j]), scratch, out)
         replaced = False
         while True:
             for _ in range(2):
@@ -1816,7 +1850,7 @@ def _block_qr_cgs2(lib, m, n, A, Q, R):
                     lib.axpy(m, -1., tmp, v)
             lib.dot(m, v, v, scratch, out)
             nrm = float(np.sqrt(max(backend.read_scalar(out), 0.)))
-            ref = 1. if replaced else col_norm[j]
+            ref = 1. if replaced else col_norm
             if nrm > 64 * np.finfo(np.float64).eps * ref and nrm > 0.:
                 break
             # dependent column: continue with a unit vector (the next one not yet tried)

@@ -88,6 +88,12 @@ def ozaki_product(a, b):
     return C
 
 
+def fro_norm(blk):
+    """|blk|_F without over- or underflow (the kernels scale every block by a power of two first)"""
+    amax = np.max(np.abs(blk), initial=0.)
+    return amax * np.linalg.norm(blk / amax) if 0. < amax < np.inf else np.linalg.norm(blk)
+
+
 class FakeDeviceLib:
     name = 'FAKE numpy test double (tests only)'
 
@@ -252,7 +258,7 @@ class FakeDeviceLib:
             k = min(mi, ni)
             blk = a[a_off[i]:a_off[i] + mi * ni].reshape(mi, ni)
             uu, ss, vv = np.linalg.svd(blk, full_matrices=False)
-            defl = max(16 * 2.220446049250313e-16 * np.sqrt(max(mi, ni)), self.deflation_tol) * np.linalg.norm(blk) \
+            defl = max(16 * 2.220446049250313e-16 * np.sqrt(max(mi, ni)), self.deflation_tol) * fro_norm(blk) \
                 if self.deflation else -1.
             r = int(np.sum(ss > defl))
             vv = vv.copy()
