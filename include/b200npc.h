@@ -184,7 +184,8 @@ int b200_scale_axis_f64(int64_t n_tasks, const int64_t *task_dev, const int64_t 
 /* Batched Householder QR: block i is A_i (m_i x n_i, row-major at A + a_off[i]); Q_i (m_i x k_i, k = min(m, n)) is
  * written to Q + q_off[i], R_i (k_i x n_i, upper triangular, non-negative diagonal) to R + r_off[i].  One CTA per block,
  * one launch, no host round trip.  replaces the per-block np.linalg.qr of npc.qr (np_conserved.py:4139).  `work` =
- * device scratch of b200_block_qr_worksize bytes.  Used for blocks up to 384 rows / columns (np_conserved.qr_method = 'auto').
+ * device scratch of b200_block_qr_worksize bytes.  npc.qr uses it for real blocks of up to 384 rows and columns
+ * (np_conserved.QR_HOUSEHOLDER_MAX).
  * Range: every finite block.  Each block is factored as 2^-e A_i, 2^e the power of two of max |a_ij| (exact), and R is
  * scaled back by 2^e: Q is bit for bit that of 2^-e A_i and R exactly 2^e times its R (rounded once where it is subnormal). */
 int64_t b200_block_qr_worksize(int64_t nblocks, const int64_t *m_host, const int64_t *n_host);
@@ -274,10 +275,11 @@ int b200_block_svd_z(int64_t nblocks, const int64_t *m_host, const int64_t *n_ho
                      int32_t *transposed_host, b200_stream_t stream);
 /* Complex counterpart of b200_block_qr_f64: Householder QR (zgeqr2 + zung2r) of complex row-major blocks, planar buffers
  * sharing one offset table; Q_i (m_i x k_i) with orthonormal columns, R_i (k_i x n_i) upper triangular with a real
- * non-negative diagonal.  One CTA per block, one launch, every block size (cost O(m n k) on one SM: meant for the
- * canonical-form path, not for large dense blocks).  replaces the per-block np.linalg.qr of npc.qr (np_conserved.py:4139)
- * for complex blocks.  `work` = device scratch of b200_block_qr_z_worksize bytes.  Range and power-of-two scaling of the
- * block: as b200_block_qr_f64 (max over the real and imaginary parts). */
+ * non-negative diagonal.  The same kernel and argument checks as b200_block_qr_f64, run with the imaginary planes.  One
+ * CTA per block, one launch, every block size (cost O(m n k) on one SM: meant for the canonical-form path, not for large
+ * dense blocks).  replaces the per-block np.linalg.qr of npc.qr (np_conserved.py:4139) for complex blocks.  `work` =
+ * device scratch of b200_block_qr_z_worksize bytes (more than b200_block_qr_worksize of the same shapes).  Range and
+ * power-of-two scaling of the block: as b200_block_qr_f64 (max over the real and imaginary parts). */
 int64_t b200_block_qr_z_worksize(int64_t nblocks, const int64_t *m_host, const int64_t *n_host);
 int b200_block_qr_z(int64_t nblocks, const int64_t *m_host, const int64_t *n_host, const int64_t *a_off_host,
                     const int64_t *q_off_host, const int64_t *r_off_host, const double *A_re, const double *A_im,

@@ -385,56 +385,28 @@ class DeviceLib:
                                                       self.stream()))
 
     # -- decompositions
-    def block_svd(self, m, n, a_off, u_off, s_off, vt_off, A, U, S, VT):
+    def _svd_call(self, fn, worksize, m, n, a_off, u_off, s_off, vt_off, A, U, S, VT):
+        """one batched block SVD through `fn` (b200_block_svd_f64 or b200_block_svd_z); A, U, VT: tuples of planes.  A batch
+        with a block that did not converge within the sweep limit (B200_ERR_NOCONV) runs once more with the conservative
+        settings (four inner sweeps of the pivot solver, every direction iterated to convergence) before giving up; A is
+        untouched.  Returns (info, nact, transposed)."""
         ms, ns, ao, uo, so, vo = [_i64(x) for x in (m, n, a_off, u_off, s_off, vt_off)]
         nb = len(ms[0])
-        wbytes = int(self.c.b200_block_svd_worksize(nb, ms[1], ns[1]))
+        wbytes = int(worksize(nb, ms[1], ns[1]))
         work = self.torch.empty(wbytes, dtype=self.torch.uint8, device=self.device)
         info = np.zeros(nb, dtype=np.int32)
         nact = np.zeros(nb, dtype=np.int32)
         transp = np.zeros(nb, dtype=np.int32)
         def call():
-            return self.c.b200_block_svd_f64(nb, ms[1], ns[1], ao[1], uo[1], so[1], vo[1], _ptr(A), _ptr(U), _ptr(S), _ptr(VT),
-                                             _ptr(work), wbytes, info.ctypes.data_as(c_i32p), nact.ctypes.data_as(c_i32p),
-                                             transp.ctypes.data_as(c_i32p), self.stream())
+            return fn(nb, ms[1], ns[1], ao[1], uo[1], so[1], vo[1], *map(_ptr, A + U + (S,) + VT), _ptr(work), wbytes,
+                      info.ctypes.data_as(c_i32p), nact.ctypes.data_as(c_i32p), transp.ctypes.data_as(c_i32p), self.stream())
         with _Prof(self, 'svd'):
             rc = call()
             if rc == B200_ERR_NOCONV:
-                # a block did not converge within the sweep limit: once more with the conservative settings (four inner
-                # sweeps of the pivot solver, every direction iterated to convergence) before giving up; A is untouched
                 self.noconv_retries += 1
                 old_in, old_defl = self.svd_set_eig_inner_sweeps(4), self.svd_set_deflation(False)
                 try:
-                    U.zero_()
-                    VT.zero_()
-                    rc = call()
-                finally:
-                    self.svd_set_eig_inner_sweeps(old_in)
-                    self.svd_set_deflation(old_defl)
-            self._check(rc)
-        return info, nact, transp
-
-    def block_svd_z(self, m, n, a_off, u_off, s_off, vt_off, A_re, A_im, U_re, U_im, S, VT_re, VT_im):
-        """complex block SVD on planar buffers (include/b200npc.h); returns (info, nact, transposed) like block_svd"""
-        ms, ns, ao, uo, so, vo = [_i64(x) for x in (m, n, a_off, u_off, s_off, vt_off)]
-        nb = len(ms[0])
-        wbytes = int(self.c.b200_block_svd_z_worksize(nb, ms[1], ns[1]))
-        work = self.torch.empty(wbytes, dtype=self.torch.uint8, device=self.device)
-        info = np.zeros(nb, dtype=np.int32)
-        nact = np.zeros(nb, dtype=np.int32)
-        transp = np.zeros(nb, dtype=np.int32)
-        def call():
-            return self.c.b200_block_svd_z(nb, ms[1], ns[1], ao[1], uo[1], so[1], vo[1], _ptr(A_re), _ptr(A_im), _ptr(U_re),
-                                           _ptr(U_im), _ptr(S), _ptr(VT_re), _ptr(VT_im), _ptr(work), wbytes,
-                                           info.ctypes.data_as(c_i32p), nact.ctypes.data_as(c_i32p),
-                                           transp.ctypes.data_as(c_i32p), self.stream())
-        with _Prof(self, 'svd'):
-            rc = call()
-            if rc == B200_ERR_NOCONV:     # as block_svd: once more with the conservative settings
-                self.noconv_retries += 1
-                old_in, old_defl = self.svd_set_eig_inner_sweeps(4), self.svd_set_deflation(False)
-                try:
-                    for t in (U_re, U_im, VT_re, VT_im):
+                    for t in U + VT:
                         t.zero_()
                     rc = call()
                 finally:
@@ -443,25 +415,34 @@ class DeviceLib:
             self._check(rc)
         return info, nact, transp
 
-    def block_qr_z(self, m, n, a_off, q_off, r_off, A_re, A_im, Q_re, Q_im, R_re, R_im):
-        """batched complex Householder QR on planar buffers (include/b200npc.h)"""
+    def block_svd(self, m, n, a_off, u_off, s_off, vt_off, A, U, S, VT):
+        """batched block SVD (include/b200npc.h); returns (info, nact, transposed)"""
+        return self._svd_call(self.c.b200_block_svd_f64, self.c.b200_block_svd_worksize, m, n, a_off, u_off, s_off,
+                              vt_off, (A,), (U,), S, (VT,))
+
+    def block_svd_z(self, m, n, a_off, u_off, s_off, vt_off, A_re, A_im, U_re, U_im, S, VT_re, VT_im):
+        """complex block SVD on planar buffers (include/b200npc.h); returns (info, nact, transposed) like block_svd"""
+        return self._svd_call(self.c.b200_block_svd_z, self.c.b200_block_svd_z_worksize, m, n, a_off, u_off, s_off,
+                              vt_off, (A_re, A_im), (U_re, U_im), S, (VT_re, VT_im))
+
+    def _qr_call(self, fn, worksize, m, n, a_off, q_off, r_off, A, Q, R):
+        """one batched Householder QR through `fn` (b200_block_qr_f64 or b200_block_qr_z); A, Q, R: tuples of planes"""
         ms, ns, ao, qo, ro = [_i64(x) for x in (m, n, a_off, q_off, r_off)]
         nb = len(ms[0])
-        wbytes = int(self.c.b200_block_qr_z_worksize(nb, ms[1], ns[1]))
+        wbytes = int(worksize(nb, ms[1], ns[1]))
         work = self.torch.empty(wbytes, dtype=self.torch.uint8, device=self.device)
         with _Prof(self, 'svd'):
-            self._check(self.c.b200_block_qr_z(nb, ms[1], ns[1], ao[1], qo[1], ro[1], _ptr(A_re), _ptr(A_im), _ptr(Q_re),
-                                               _ptr(Q_im), _ptr(R_re), _ptr(R_im), _ptr(work), wbytes, self.stream()))
+            self._check(fn(nb, ms[1], ns[1], ao[1], qo[1], ro[1], *map(_ptr, A + Q + R), _ptr(work), wbytes,
+                           self.stream()))
 
     def block_qr(self, m, n, a_off, q_off, r_off, A, Q, R):
         """batched Householder QR of the blocks (include/b200npc.h)"""
-        ms, ns, ao, qo, ro = [_i64(x) for x in (m, n, a_off, q_off, r_off)]
-        nb = len(ms[0])
-        wbytes = int(self.c.b200_block_qr_worksize(nb, ms[1], ns[1]))
-        work = self.torch.empty(wbytes, dtype=self.torch.uint8, device=self.device)
-        with _Prof(self, 'svd'):
-            self._check(self.c.b200_block_qr_f64(nb, ms[1], ns[1], ao[1], qo[1], ro[1], _ptr(A), _ptr(Q), _ptr(R),
-                                                 _ptr(work), wbytes, self.stream()))
+        self._qr_call(self.c.b200_block_qr_f64, self.c.b200_block_qr_worksize, m, n, a_off, q_off, r_off, (A,), (Q,), (R,))
+
+    def block_qr_z(self, m, n, a_off, q_off, r_off, A_re, A_im, Q_re, Q_im, R_re, R_im):
+        """batched complex Householder QR on planar buffers (include/b200npc.h)"""
+        self._qr_call(self.c.b200_block_qr_z, self.c.b200_block_qr_z_worksize, m, n, a_off, q_off, r_off, (A_re, A_im),
+                      (Q_re, Q_im), (R_re, R_im))
 
     def col_sqnorms(self, rows, cols, ld, X, OUT):
         with _Prof(self, 'svd'):
@@ -482,7 +463,8 @@ class DeviceLib:
         return int(self.c.b200_svd_set_fused_max_ld(int(max_ld)))
 
     def svd_set_eig_variant(self, variant):
-        """1 = jacobi_eig_kernel (default), 2 = jacobi_eig_kernel_v2; returns the old value"""
+        """pivot eigen-solver of the Jacobi rounds: 1 = jacobi_eig_kernel, 3 = jacobi_eig_kernel_v3 (default); other values
+        leave it unchanged; returns the old value"""
         return int(self.c.b200_svd_set_eig_variant(int(variant)))
 
     def block_eigh(self, n, a_off, w_off, v_off, A, W, V):

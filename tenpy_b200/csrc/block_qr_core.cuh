@@ -7,6 +7,12 @@
 // charge-conserving tensors, one launch per Array with no host round trip; big dense blocks want the blocked (compact WY)
 // multi-CTA version -- round-2 work together with the QR preconditioning of the Jacobi SVD (DESIGN.md section 8).
 //
+// Complex blocks are planar: every phase takes the imaginary planes (Ai, Vi, Qi, ...) as trailing arguments, NULL (the
+// default) for a real block.  The complex case is zgeqr2 + zung2r: reflector j is H_j = 1 - tau_j v v^H with v[j] = 1,
+// complex tau and a real beta (zlarfg), A <- H_j^H A, Q = H_0 H_1 ... H_{k-1} applied to the first k columns of the
+// identity; the diagonal of R is real by construction.  With the imaginary planes NULL every phase does exactly the real
+// operations.
+//
 // Threads own COLUMNS (row-major storage: for a fixed row, consecutive threads touch consecutive addresses); the only
 // cross-thread quantity per Householder step is the squared norm of the pivot column below the diagonal, summed in a
 // fixed order from per-thread partials (deterministic).  Every phase is a plain function of (tid, nthreads, pointers):
@@ -46,92 +52,158 @@ BQ_HD double block_scale(int T, const double *partial) {
     return b200::pow2_scale(a);
 }
 
-// PHASE 0 (after block_scale): A[e] = A_in[e] * scale, the working copy the factorisation runs on
-BQ_HD void scale_in(int tid, int T, const double *A_in, double *A, int64_t len, double scale) {
-    for (int64_t e = tid; e < len; e += T) A[e] = A_in[e] * scale;
+// PHASE 0 (after block_scale): A[e] = A_in[e] * scale (and Ai from Ai_in), the working copy the factorisation runs on
+BQ_HD void scale_in(int tid, int T, const double *A_in, double *A, int64_t len, double scale,
+                    const double *Ai_in = nullptr, double *Ai = nullptr) {
+    for (int64_t e = tid; e < len; e += T) {
+        A[e] = A_in[e] * scale;
+        if (Ai) Ai[e] = Ai_in[e] * scale;
+    }
 }
 
-// LAST PHASE: R_out = the first k rows of A times rscale = 1 / scale (exact: a power of two)
-BQ_HD void store_r(int tid, int T, const double *A, double *R_out, int k, int n, double rscale) {
-    for (int64_t e = tid; e < (int64_t)k * n; e += T) R_out[e] = A[e] * rscale;
+// LAST PHASE: R_out = the first k rows of A times rscale = 1 / scale (exact: a power of two); Ri_out from Ai
+BQ_HD void store_r(int tid, int T, const double *A, double *R_out, int k, int n, double rscale,
+                   const double *Ai = nullptr, double *Ri_out = nullptr) {
+    for (int64_t e = tid; e < (int64_t)k * n; e += T) {
+        R_out[e] = A[e] * rscale;
+        if (Ai) Ri_out[e] = Ai[e] * rscale;
+    }
 }
 
-// PHASE 1: partial[tid] = sum over rows r > j (strided by threads) of A[r][j]^2
-BQ_HD void col_partial(int tid, int T, const double *A, int m, int n, int j, double *partial) {
+// PHASE 1: partial[tid] = sum over rows r > j (strided by threads) of |A[r][j]|^2
+BQ_HD void col_partial(int tid, int T, const double *A, int m, int n, int j, double *partial,
+                       const double *Ai = nullptr) {
     double s = 0.0;
     for (int r = j + 1 + tid; r < m; r += T) {
         const double a = A[(int64_t)r * n + j];
-        s = fma(a, a, s);
+        if (Ai) {
+            const double b = Ai[(int64_t)r * n + j];
+            s = fma(a, a, fma(b, b, s));
+        } else {
+            s = fma(a, a, s);
+        }
     }
     partial[tid] = s;
 }
 
-// PHASE 2 (one thread): reflector H = 1 - tau v v^T with v[j] = 1 that maps the pivot column to beta e_j.
-// params[0] = tau, params[1] = scale (v[r] = A[r][j] * scale for r > j), params[2] = beta
-BQ_HD void reflector(int T, const double *A, int n, int j, const double *partial, double *params) {
+// PHASE 2 (one thread): reflector H = 1 - tau v v^H with v[j] = 1 that maps the pivot column to beta e_j (H^H for a
+// complex block), beta real: beta = -sign(Re alpha) |column from the diagonal down|, tau = (beta - alpha) / beta,
+// scale = 1 / (alpha - beta).  params[0] = Re tau, params[1] = Re scale (v[r] = A[r][j] * scale for r > j),
+// params[2] = beta; a complex block (Ai not NULL) also writes params[3] = Im tau, params[4] = Im scale
+BQ_HD void reflector(int T, const double *A, int n, int j, const double *partial, double *params,
+                     const double *Ai = nullptr) {
     double sigma = 0.0;
     for (int t = 0; t < T; ++t) sigma += partial[t];
-    const double alpha = A[(int64_t)j * n + j];
-    if (sigma == 0.0) {
+    const double alpha = A[(int64_t)j * n + j], ai = Ai ? Ai[(int64_t)j * n + j] : 0.0;
+    if (Ai) params[3] = params[4] = 0.0;
+    if (sigma == 0.0 && ai == 0.0) {                  // H = 1
         params[0] = 0.0;
         params[1] = 0.0;
         params[2] = alpha;
-    } else {
-        const double nrm = sqrt(alpha * alpha + sigma);
-        const double beta = alpha >= 0.0 ? -nrm : nrm;
-        params[0] = (beta - alpha) / beta;
-        params[1] = 1.0 / (alpha - beta);
-        params[2] = beta;
+        return;
     }
+    const double nrm = Ai ? sqrt(fma(alpha, alpha, fma(ai, ai, sigma))) : sqrt(alpha * alpha + sigma);
+    const double beta = alpha >= 0.0 ? -nrm : nrm;
+    params[0] = (beta - alpha) / beta;
+    if (Ai) {
+        params[3] = -ai / beta;
+        const double dr = alpha - beta, di = ai, d2 = dr * dr + di * di;
+        params[1] = dr / d2;
+        params[4] = -di / d2;
+    } else {
+        params[1] = 1.0 / (alpha - beta);
+    }
+    params[2] = beta;
 }
 
 // PHASE 3: store the reflector: V[r][j] = A[r][j] * scale (r > j), V[j][j] = 1, V[r][j] = 0 (r < j); A[r][j] = 0 below
-// the diagonal, A[j][j] = beta.  V is m x k row-major.
-BQ_HD void store_reflector(int tid, int T, double *A, double *V, int m, int n, int k, int j, const double *params) {
-    const double scale = params[1];
+// the diagonal, A[j][j] = beta.  V (and Vi) is m x k row-major.
+BQ_HD void store_reflector(int tid, int T, double *A, double *V, int m, int n, int k, int j, const double *params,
+                           double *Ai = nullptr, double *Vi = nullptr) {
+    const double scr = params[1], sci = Ai ? params[4] : 0.0;
     for (int r = tid; r < m; r += T) {
-        double v = 0.0;
+        double vr = 0.0, vi = 0.0;
         if (r == j) {
-            v = 1.0;
+            vr = 1.0;
             A[(int64_t)r * n + j] = params[2];
+            if (Ai) Ai[(int64_t)r * n + j] = 0.0;
         } else if (r > j) {
-            v = A[(int64_t)r * n + j] * scale;
-            A[(int64_t)r * n + j] = 0.0;
+            const int64_t o = (int64_t)r * n + j;
+            if (Ai) {
+                vr = A[o] * scr - Ai[o] * sci;
+                vi = A[o] * sci + Ai[o] * scr;
+                Ai[o] = 0.0;
+            } else {
+                vr = A[o] * scr;
+            }
+            A[o] = 0.0;
         }
-        V[(int64_t)r * k + j] = v;
+        V[(int64_t)r * k + j] = vr;
+        if (Vi) Vi[(int64_t)r * k + j] = vi;
     }
 }
 
-// PHASE 4: apply H to the columns c > j of X (ld = ncol; X = A with c0 = j + 1, or X = Q with c0 = j): every thread owns
-// columns c = c0 + tid, c0 + tid + T, ...:  w = sum_{r >= j} V[r][j] X[r][c];  X[r][c] -= tau V[r][j] w
-BQ_HD void apply_reflector(int tid, int T, double *X, int ncol, const double *V, int m, int k, int j, int c0, double tau) {
-    if (tau == 0.0) return;
+// PHASE 4: apply 1 - t v v^H (t = tau + i ti) to the columns c >= c0 of X (ld = ncol; X = A with t = conj(tau) and
+// c0 = j + 1, or X = Q with t = tau and c0 = j): every thread owns columns c = c0 + tid, c0 + tid + T, ...:
+// w = sum_{r >= j} conj(V[r][j]) X[r][c];  X[r][c] -= t w V[r][j]
+BQ_HD void apply_reflector(int tid, int T, double *X, int ncol, const double *V, int m, int k, int j, int c0, double tau,
+                           double *Xi = nullptr, const double *Vi = nullptr, double ti = 0.0) {
+    if (tau == 0.0 && ti == 0.0) return;
+    if (!Xi) {
+        for (int c = c0 + tid; c < ncol; c += T) {
+            double w = 0.0;
+            for (int r = j; r < m; ++r) w = fma(V[(int64_t)r * k + j], X[(int64_t)r * ncol + c], w);
+            w *= tau;
+            for (int r = j; r < m; ++r) X[(int64_t)r * ncol + c] = fma(-V[(int64_t)r * k + j], w, X[(int64_t)r * ncol + c]);
+        }
+        return;
+    }
+    const double tr = tau;
     for (int c = c0 + tid; c < ncol; c += T) {
-        double w = 0.0;
-        for (int r = j; r < m; ++r) w = fma(V[(int64_t)r * k + j], X[(int64_t)r * ncol + c], w);
-        w *= tau;
-        for (int r = j; r < m; ++r) X[(int64_t)r * ncol + c] = fma(-V[(int64_t)r * k + j], w, X[(int64_t)r * ncol + c]);
+        double wr = 0.0, wi = 0.0;
+        for (int r = j; r < m; ++r) {
+            const double vr = V[(int64_t)r * k + j], vi = Vi[(int64_t)r * k + j];
+            const double xr = X[(int64_t)r * ncol + c], xi = Xi[(int64_t)r * ncol + c];
+            wr = fma(vr, xr, fma(vi, xi, wr));
+            wi = fma(vr, xi, fma(-vi, xr, wi));
+        }
+        const double fr = tr * wr - ti * wi, fi = tr * wi + ti * wr;
+        for (int r = j; r < m; ++r) {
+            const double vr = V[(int64_t)r * k + j], vi = Vi[(int64_t)r * k + j];
+            X[(int64_t)r * ncol + c] -= fr * vr - fi * vi;
+            Xi[(int64_t)r * ncol + c] -= fr * vi + fi * vr;
+        }
     }
 }
 
 // PHASE Q0: Q = first k columns of the identity
-BQ_HD void init_q(int tid, int T, double *Q, int m, int k) {
-    for (int64_t e = tid; e < (int64_t)m * k; e += T) Q[e] = (e / k == e % k) ? 1.0 : 0.0;
+BQ_HD void init_q(int tid, int T, double *Q, int m, int k, double *Qi = nullptr) {
+    for (int64_t e = tid; e < (int64_t)m * k; e += T) {
+        Q[e] = (e / k == e % k) ? 1.0 : 0.0;
+        if (Qi) Qi[e] = 0.0;
+    }
 }
 
-// PHASE S: make diag(R) non-negative: rows i of R (= A) and columns i of Q with R[i][i] < 0 change sign.
+// PHASE S: make diag(R) non-negative (it is real): rows i of R (= A) and columns i of Q with R[i][i] < 0 change sign.
 // sign[i] must have been written by the previous phase (sign_of_diag).
 BQ_HD void sign_of_diag(int tid, int T, const double *A, int n, int k, double *sign) {
     for (int i = tid; i < k; i += T) sign[i] = A[(int64_t)i * n + i] < 0.0 ? -1.0 : 1.0;
 }
-BQ_HD void flip_signs(int tid, int T, double *A, double *Q, int m, int n, int k, const double *sign) {
+BQ_HD void flip_signs(int tid, int T, double *A, double *Q, int m, int n, int k, const double *sign,
+                      double *Ai = nullptr, double *Qi = nullptr) {
     for (int64_t e = tid; e < (int64_t)k * n; e += T) {
         const int i = (int)(e / n);
-        if (sign[i] < 0.0) A[e] = -A[e];
+        if (sign[i] < 0.0) {
+            A[e] = -A[e];
+            if (Ai) Ai[e] = -Ai[e];
+        }
     }
     for (int64_t e = tid; e < (int64_t)m * k; e += T) {
         const int i = (int)(e % k);
-        if (sign[i] < 0.0) Q[e] = -Q[e];
+        if (sign[i] < 0.0) {
+            Q[e] = -Q[e];
+            if (Qi) Qi[e] = -Qi[e];
+        }
     }
 }
 

@@ -1184,38 +1184,14 @@ __global__ void __launch_bounds__(1024) jacobi_reorder_kernel(const double *__re
     }
 }
 
-// SVD finalize: grid (max_k, nmat)
-__global__ void __launch_bounds__(128)
-    svd_finalize_kernel(const double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ perm,
-                        double *__restrict__ U, double *__restrict__ S, double *__restrict__ VT) {
-    const JMat mt = mats[blockIdx.y];
-    const int r = blockIdx.x;
-    const int k = mt.q;
-    if (r >= k) return;
-    const int src = perm[mt.perm_off + r];
-    const double s = work[mt.snorm_off + src];
-    const double inv = (s > mt.defl && s > 0.0) ? 1.0 / s : 0.0;   // negligible direction: filled by the caller
-    const double *y = work + mt.y_off + (int64_t)src * mt.ldy;
-    const double *w = work + mt.w_off + (int64_t)src * mt.ldw;
-    if (threadIdx.x == 0) S[mt.s_off + r] = s / mt.scale;     // exact: scale is a power of two
-    double *u = U + mt.u_off;
-    double *vt = VT + mt.vt_off;
-    if (mt.transposed) {  // Y rows: length m -> U[:, r];  W rows: length n -> VT[r, :]
-        for (int i = threadIdx.x; i < mt.m; i += blockDim.x) u[(int64_t)i * k + r] = y[i] * inv;
-        for (int c = threadIdx.x; c < mt.n; c += blockDim.x) vt[(int64_t)r * mt.n + c] = w[c];
-    } else {  // Y rows: length n -> VT[r, :];  W rows: length m -> U[:, r]
-        for (int c = threadIdx.x; c < mt.n; c += blockDim.x) vt[(int64_t)r * mt.n + c] = y[c] * inv;
-        for (int i = threadIdx.x; i < mt.m; i += blockDim.x) u[(int64_t)i * k + r] = w[i];
-    }
-}
-
-// complex SVD finalize: grid (max_k, nmat).  W Y0 = Y with W unitary and the rows of Y orthogonal:
+// SVD finalize: grid (max_k, nmat).  W Y0 = Y with W orthogonal (unitary) and the rows of Y orthogonal:
 //   not transposed (Y0 = A):    A = W^H Y        -> U[:, r] = conj(W[r, :]),  VT[r, :] = Y[r, :] / s_r
 //   transposed (Y0 = A^T):      A = Y^T conj(W)  -> U[:, r] = Y[r, :] / s_r,  VT[r, :] = conj(W[r, :])
+// Ui, VTi (complex matrices, else NULL): the imaginary parts, from Yi and Wi
 __global__ void __launch_bounds__(128)
-    zsvd_finalize_kernel(const double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ perm,
-                         double *__restrict__ Ur, double *__restrict__ Ui, double *__restrict__ S,
-                         double *__restrict__ VTr, double *__restrict__ VTi) {
+    svd_finalize_kernel(const double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ perm,
+                        double *__restrict__ U, double *__restrict__ Ui, double *__restrict__ S, double *__restrict__ VT,
+                        double *__restrict__ VTi) {
     const JMat mt = mats[blockIdx.y];
     const int r = blockIdx.x;
     const int k = mt.q;
@@ -1223,26 +1199,27 @@ __global__ void __launch_bounds__(128)
     const int src = perm[mt.perm_off + r];
     const double s = work[mt.snorm_off + src];
     const double inv = (s > mt.defl && s > 0.0) ? 1.0 / s : 0.0;   // negligible direction: filled by the caller
-    const double *yr = work + mt.y_off + (int64_t)src * mt.ldy, *yi = work + mt.yi_off + (int64_t)src * mt.ldy;
-    const double *wr = work + mt.w_off + (int64_t)src * mt.ldw, *wi = work + mt.wi_off + (int64_t)src * mt.ldw;
+    const double *y = work + mt.y_off + (int64_t)src * mt.ldy, *yi = work + mt.yi_off + (int64_t)src * mt.ldy;
+    const double *w = work + mt.w_off + (int64_t)src * mt.ldw, *wi = work + mt.wi_off + (int64_t)src * mt.ldw;
     if (threadIdx.x == 0) S[mt.s_off + r] = s / mt.scale;     // exact: scale is a power of two
-    if (mt.transposed) {
+    const int64_t u0 = mt.u_off + r, vt0 = mt.vt_off + (int64_t)r * mt.n;
+    if (mt.transposed) {  // Y rows: length m -> U[:, r];  W rows: length n -> VT[r, :]
         for (int i = threadIdx.x; i < mt.m; i += blockDim.x) {
-            Ur[mt.u_off + (int64_t)i * k + r] = yr[i] * inv;
-            Ui[mt.u_off + (int64_t)i * k + r] = yi[i] * inv;
+            U[u0 + (int64_t)i * k] = y[i] * inv;
+            if (Ui) Ui[u0 + (int64_t)i * k] = yi[i] * inv;
         }
         for (int c = threadIdx.x; c < mt.n; c += blockDim.x) {
-            VTr[mt.vt_off + (int64_t)r * mt.n + c] = wr[c];
-            VTi[mt.vt_off + (int64_t)r * mt.n + c] = -wi[c];
+            VT[vt0 + c] = w[c];
+            if (VTi) VTi[vt0 + c] = -wi[c];
         }
-    } else {
+    } else {  // Y rows: length n -> VT[r, :];  W rows: length m -> U[:, r]
         for (int c = threadIdx.x; c < mt.n; c += blockDim.x) {
-            VTr[mt.vt_off + (int64_t)r * mt.n + c] = yr[c] * inv;
-            VTi[mt.vt_off + (int64_t)r * mt.n + c] = yi[c] * inv;
+            VT[vt0 + c] = y[c] * inv;
+            if (VTi) VTi[vt0 + c] = yi[c] * inv;
         }
         for (int i = threadIdx.x; i < mt.m; i += blockDim.x) {
-            Ur[mt.u_off + (int64_t)i * k + r] = wr[i];
-            Ui[mt.u_off + (int64_t)i * k + r] = -wi[i];
+            U[u0 + (int64_t)i * k] = w[i];
+            if (Ui) Ui[u0 + (int64_t)i * k] = -wi[i];
         }
     }
 }
@@ -1740,12 +1717,8 @@ static int block_svd_impl(int64_t nblocks, const int64_t *m, const int64_t *n, c
     std::vector<int> perm;
     rc = sort_norms(L, work, st, false, perm);
     if (rc) return rc;
-    if (cplx)
-        zsvd_finalize_kernel<<<dim3((unsigned)std::max(1, L.max_q), (unsigned)nmat), 128, 0, st>>>(
-            wf, d_mats, reinterpret_cast<int *>(work + L.off_perm), U, Ui, S, VT, VTi);
-    else
-        svd_finalize_kernel<<<dim3((unsigned)std::max(1, L.max_q), (unsigned)nmat), 128, 0, st>>>(
-            wf, d_mats, reinterpret_cast<int *>(work + L.off_perm), U, S, VT);
+    svd_finalize_kernel<<<dim3((unsigned)std::max(1, L.max_q), (unsigned)nmat), 128, 0, st>>>(
+        wf, d_mats, reinterpret_cast<int *>(work + L.off_perm), U, Ui, S, VT, VTi);
     B200_CHECK_LAUNCH();
     B200_CUDA_CHECK(cudaStreamSynchronize(st));
     if (dbg)

@@ -1540,36 +1540,31 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
         info, nact, transp = lib.block_svd(m, n, lay.offsets, u_off, s_off[:-1], v_off, a._buf, bufU, bufS, bufV)
     svd_stats['calls'] += 1
     svd_stats['jacobi_sweeps'].append(int(np.max(info)))
-    if cplx and np.any(nact < k):
-        # complete the zero vectors of the negligible directions in complex arithmetic (QR kernel, cannot fail)
+    if np.any(nact < k):
+        # numerically rank-deficient blocks: the kernel left the vectors of the negligible directions on one side zero;
+        # complete them to an orthonormal basis (LAPACK returns a complete basis, reference npc:4950).  Real blocks: GEMM-only
+        # Newton-Schulz, which can fail on an ill-conditioned start; complex blocks: the complex QR kernel, which cannot
+        if cplx:
+            fill, fill_U, fill_V = _fill_null_vectors_z, (bufU, bufU_im), (bufV, bufV_im)
+        else:
+            fill, fill_U, fill_V = _fill_null_vectors, bufU, bufV
         S_h = backend.to_host(bufS).copy()
-        for i in np.nonzero(nact < k)[0]:
-            k_fill = int(k[i]) if n_keep is None else min(int(k[i]), max(int(n_keep), int(nact[i])))
-            n_fill = k_fill - int(nact[i])
-            if n_fill > 0:
-                _fill_null_vectors_z(lib, int(m[i]), int(n[i]), int(k[i]), int(nact[i]), n_fill, bool(transp[i]),
-                                     (bufU, bufU_im), int(u_off[i]), (bufV, bufV_im), int(v_off[i]))
-            lo, hi = int(s_off[i]) + int(nact[i]), int(s_off[i]) + int(k[i])
-            S_h[lo:lo + n_fill] = np.maximum(S_h[lo:lo + n_fill], _completion_floor(S_h[int(s_off[i]):lo]))
-            S_h[lo + n_fill:hi] = 0.
-        svd_stats['completions'] = svd_stats.get('completions', 0) + 1
-        bufS = backend.to_device(S_h)
-    elif np.any(nact < k):
-        # numerically rank-deficient blocks: the kernel left the vectors of the negligible directions on one side
-        # zero; complete them to an orthonormal basis (LAPACK returns a complete basis, reference npc:4950)
-        n_fill = np.zeros(len(k), dtype=np.int64)
         try:
             for i in np.nonzero(nact < k)[0]:
                 # the caller keeps at most `n_keep` vectors in total (svd_theta: chi_max): no need to complete more
                 k_fill = int(k[i]) if n_keep is None else min(int(k[i]), max(int(n_keep), int(nact[i])))
-                n_fill[i] = k_fill - int(nact[i])
-                if n_fill[i] > 0:
-                    _fill_null_vectors(lib, int(m[i]), int(n[i]), int(k[i]), int(nact[i]), int(n_fill[i]),
-                                       bool(transp[i]), bufU, int(u_off[i]), bufV, int(v_off[i]))
-            svd_stats['completions'] = svd_stats.get('completions', 0) + 1
+                n_fill = k_fill - int(nact[i])
+                if n_fill > 0:
+                    fill(lib, int(m[i]), int(n[i]), int(k[i]), int(nact[i]), n_fill, bool(transp[i]), fill_U, int(u_off[i]),
+                         fill_V, int(v_off[i]))
+                # singular values of the negligible directions: tiny but positive for the completed vectors (so that a
+                # truncation prefers them), exactly zero for the ones left without a vector
+                lo, hi = int(s_off[i]) + int(nact[i]), int(s_off[i]) + int(k[i])
+                S_h[lo:lo + n_fill] = np.maximum(S_h[lo:lo + n_fill], _completion_floor(S_h[int(s_off[i]):lo]))
+                S_h[lo + n_fill:hi] = 0.
         except _CompletionFailed:
+            # real blocks only: decompose once more without deflation, every direction iterated to convergence
             svd_stats['completion_fallbacks'] = svd_stats.get('completion_fallbacks', 0) + 1
-            n_fill = None
             old = lib.svd_set_deflation(False)
             try:
                 bufU.zero_()
@@ -1577,15 +1572,8 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
                 info, nact, transp = lib.block_svd(m, n, lay.offsets, u_off, s_off[:-1], v_off, a._buf, bufU, bufS, bufV)
             finally:
                 lib.svd_set_deflation(old)
-        if n_fill is not None:
-            # singular values of the negligible directions: tiny but positive for the completed vectors (so that a
-            # truncation prefers them), exactly zero for the ones left without a vector
-            S_h = backend.to_host(bufS).copy()
-            for i in np.nonzero(nact < k)[0]:
-                lo, hi = int(s_off[i]) + int(nact[i]), int(s_off[i]) + int(k[i])
-                mid = lo + int(n_fill[i])
-                S_h[lo:mid] = np.maximum(S_h[lo:mid], _completion_floor(S_h[int(s_off[i]):lo]))
-                S_h[mid:hi] = 0.
+        else:
+            svd_stats['completions'] = svd_stats.get('completions', 0) + 1
             bufS = backend.to_device(S_h)
     S = backend.to_host(bufS)
     if np.any(np.isnan(S)):
@@ -1786,10 +1774,8 @@ def _complex_planes(a):
 
 
 qr_stats = {'calls': 0, 'columns': 0, 'replaced': 0}   # diagnostics of the Gram-Schmidt QR
-# 'householder': b200_block_qr_f64, one CTA per block, one launch for all blocks; 'cgs2': Gram-Schmidt on the GEMM /
-# BLAS-1 kernels (one host round trip per column); 'auto' (default): Householder for blocks up to QR_HOUSEHOLDER_MAX rows
-# or columns, Gram-Schmidt above.
-qr_method = 'auto'
+# real blocks of up to QR_HOUSEHOLDER_MAX rows and columns: b200_block_qr_f64, one CTA per block, one launch for all of
+# them; larger real blocks: Gram-Schmidt on the GEMM / BLAS-1 kernels (one host round trip per column)
 QR_HOUSEHOLDER_MAX = 384
 
 
@@ -1883,9 +1869,10 @@ def qr(a, mode='reduced', inner_labels=[None, None], cutoff=None, pos_diag_R=Fal
     """Q-R decomposition ``a == tensordot(Q, R, axes=1)`` per charge block (reference npc:4139): `Q` an isometry with
     legs ``(a.legs[0], inner.conj())``, `R` upper triangular with legs ``(inner, a.legs[1])``.
 
-    Only ``mode='reduced'`` and ``cutoff=None``.  The diagonal of `R` is positive by construction (Gram-Schmidt, see
-    :func:`_block_qr_cgs2`), i.e. the result is the unique decomposition the reference returns for
-    ``pos_diag_R=True`` (for full-rank blocks).  A :class:`ComplexArray` `a` goes through the complex Householder kernel
+    Only ``mode='reduced'`` and ``cutoff=None``.  The diagonal of `R` is non-negative by construction (Householder kernel
+    ``b200_block_qr_f64`` for blocks of up to `QR_HOUSEHOLDER_MAX` rows and columns, Gram-Schmidt :func:`_block_qr_cgs2`
+    above), i.e. the result is the unique decomposition the reference returns for ``pos_diag_R=True`` (for full-rank
+    blocks).  A :class:`ComplexArray` `a` goes through the complex Householder kernel
     (``b200_block_qr_z``, every block size); `Q` and `R` are then ComplexArrays, the diagonal of `R` real and >= 0."""
     if a.rank != 2:
         raise ValueError('expect a matrix!')
@@ -1942,16 +1929,14 @@ def qr(a, mode='reduced', inner_labels=[None, None], cutoff=None, pos_diag_R=Fal
             Q_im._set_blocks(lay_Q, bufQ_im)
             R_im._set_blocks(lay_R, bufR_im)
         else:
-            small = np.ones(lay.nblocks, bool) if qr_method == 'householder' else \
-                (np.maximum(m, n) <= QR_HOUSEHOLDER_MAX if qr_method == 'auto' else np.zeros(lay.nblocks, bool))
+            small = np.maximum(m, n) <= QR_HOUSEHOLDER_MAX
             if np.any(small):
                 lib.block_qr(m[small], n[small], lay.offsets[small], q_off[small], r_off[small], a._buf, bufQ, bufR)
-            if not np.all(small):
-                for b in np.nonzero(~small)[0]:
-                    mb, nb, kb = int(m[b]), int(n[b]), int(k[b])
-                    ao = int(lay.offsets[b])
-                    _block_qr_cgs2(lib, mb, nb, a._buf[ao:ao + mb * nb], bufQ[int(q_off[b]):int(q_off[b]) + mb * kb],
-                                   bufR[int(r_off[b]):int(r_off[b]) + kb * nb])
+            for b in np.nonzero(~small)[0]:
+                mb, nb, kb = int(m[b]), int(n[b]), int(k[b])
+                ao = int(lay.offsets[b])
+                _block_qr_cgs2(lib, mb, nb, a._buf[ao:ao + mb * nb], bufQ[int(q_off[b]):int(q_off[b]) + mb * kb],
+                               bufR[int(r_off[b]):int(r_off[b]) + kb * nb])
         Q._set_blocks(lay_Q, bufQ)
         R._set_blocks(lay_R, bufR)
         qr_stats['calls'] += 1

@@ -93,17 +93,33 @@ def test_qr_host_logic(fake_device):
     _check_qr()
 
 
-def test_qr_householder_route_host_logic(fake_device):
-    """np_conserved.qr_method = 'householder' (b200_block_qr_f64: all blocks in one launch) gives the same factors"""
+def test_qr_block_size_route_host_logic(fake_device):
+    """npc.qr of an Array with one block of at most QR_HOUSEHOLDER_MAX rows and columns and one above: the small block goes
+    through b200_block_qr_f64, the large one through Gram-Schmidt; both give numpy's factors (diagonal of R made
+    non-negative) to the tolerances of _check_qr"""
     from tenpy_b200.linalg import np_conserved as npc
-    old = npc.qr_method
-    npc.qr_method = 'householder'
-    try:
-        n0 = fake_device.calls.get('block_qr', 0)
-        _check_qr()
-        assert fake_device.calls.get('block_qr', 0) > n0
-    finally:
-        npc.qr_method = old
+    ci = npc.ChargeInfo([1], ['N'])
+    lL = npc.LegCharge.from_qind(ci, [0, 7, 407], [[0], [1]], +1)
+    lR = npc.LegCharge.from_qind(ci, [0, 5, 8], [[0], [1]], -1)
+    rng = np.random.default_rng(8)
+    blocks = [rng.standard_normal((7, 5)), rng.standard_normal((400, 3))]
+    assert max(blocks[0].shape) <= npc.QR_HOUSEHOLDER_MAX < max(blocks[1].shape)
+    a = npc.Array.from_blocks([lL, lR], [[0, 0], [1, 1]], blocks, None, ['a', 'b'])
+    n_qr, n_cols = fake_device.calls.get('block_qr', 0), npc.qr_stats['columns']
+    Q, R = npc.qr(a, inner_labels=['q', 'r'])
+    assert fake_device.calls.get('block_qr', 0) == n_qr + 1        # the small block: one Householder launch
+    assert npc.qr_stats['columns'] == n_cols + 3                    # the large block: Gram-Schmidt, 3 columns
+    q, r = Q.to_ndarray(), R.to_ndarray()
+    rows, cols, segs = a.legs[0].slices, a.legs[1].slices, Q.legs[1].slices
+    for i, A in enumerate(blocks):
+        qb = q[rows[i]:rows[i + 1], segs[i]:segs[i + 1]]
+        rb = r[segs[i]:segs[i + 1], cols[i]:cols[i + 1]]
+        qq, rr = np.linalg.qr(A)
+        sgn = np.where(np.diag(rr) < 0., -1., 1.)
+        assert np.max(np.abs(qb - qq * sgn[None, :])) < 1e-12 and np.max(np.abs(rb - rr * sgn[:, None])) < 1e-12, i
+        assert np.max(np.abs(qb @ rb - A)) < 1e-13 * np.abs(A).max() * max(A.shape), i
+        assert np.max(np.abs(qb.T @ qb - np.eye(min(A.shape)))) < 1e-13, i
+        assert np.all(np.tril(rb, -1) == 0.) and np.all(np.diag(rb) > 0.), i
 
 
 @pytest.mark.gpu

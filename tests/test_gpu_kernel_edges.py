@@ -81,8 +81,9 @@ def _qr_inputs(rng):
 
 
 def test_block_qr_batch(gpu_lib):
-    """b200_block_qr_f64 (np_conserved.qr_method = 'auto' sends every block <= 384 here) on one batch of edge shapes:
-    Q^T Q = 1, R upper triangular with a non-negative diagonal, QR = A, and Q, R equal LAPACK's after the sign fix"""
+    """b200_block_qr_f64 (npc.qr sends every real block <= np_conserved.QR_HOUSEHOLDER_MAX = 384 here) on one batch of
+    edge shapes: Q^T Q = 1, R upper triangular with a non-negative diagonal, QR = A, and Q, R equal LAPACK's after the
+    sign fix"""
     rng = np.random.default_rng(101)
     mats = _qr_inputs(rng)
     ms = [a.shape[0] for _, a, _ in mats]

@@ -1,7 +1,8 @@
 """Host run of the Householder QR phases (tests/csrc/block_qr_host.cpp): the phases of block_qr_core.cuh executed for
-every thread index exactly as block_qr_kernel executes them, compiled with the host C++ compiler.  Checks QR = A,
-orthonormal Q and triangular R at edge shapes, and exact power-of-two equivariance of Q and R for 2^e A with
-|e| <= 990.  No GPU needed; skipped where no C++ compiler is installed."""
+every thread index exactly as block_qr_kernel executes them, compiled with the host C++ compiler, for real and for
+complex blocks.  Checks QR = A, orthonormal Q and triangular R with a real non-negative diagonal at edge shapes, and
+exact power-of-two equivariance of Q and R for 2^e A with |e| <= 990.  No GPU needed; skipped where no C++ compiler is
+installed."""
 import os
 import shutil
 import subprocess
@@ -20,4 +21,7 @@ def test_block_qr_host_phases(tmp_path):
                    check=True)
     res = subprocess.run([exe], capture_output=True, text=True, timeout=600)
     assert res.returncode == 0, res.stdout + res.stderr
-    assert 'scale cases: ok' in res.stdout
+    lines = res.stdout.splitlines()
+    assert 'scale cases: ok' in lines
+    assert 'complex scale cases: ok' in lines
+    assert lines[-1] == 'ok'
