@@ -234,8 +234,9 @@ int b200_col_sqnorms_f64(int64_t rows, int64_t cols, int64_t ld, const double *X
  * replaces _svd_worker npc:4950 -> svd_robust.svd svd_robust.py:37 (LAPACK gesdd / gesvd). */
 /* switch the deflation of negligible directions in b200_block_svd_f64 on (default) / off; returns the old value */
 int b200_svd_set_deflation(int on);
-/* pivot eigen-solver of the Jacobi rounds: 1 = jacobi_eig_kernel (G in shared memory, three barriers per rotation set),
- * 3 = jacobi_eig_kernel_v3 (G and Q in registers, warp shuffles, two barriers per set); returns the old value */
+/* pivot eigen-solver of the real Jacobi rounds: 1 = jacobi_eig_kernel<false> (G in shared memory, three barriers per
+ * rotation set), 3 = jacobi_eig_kernel_v3 (G and Q in registers, warp shuffles, two barriers per set); complex rounds
+ * always use jacobi_eig_kernel<true>.  Returns the old value */
 int b200_svd_set_eig_variant(int variant);
 /* inner sweeps of the version-3 pivot eigen-solver (1..16, default 2): profiles/jacobi_sweeps_study.md finds the number
  * of outer sweeps unchanged between 2 and 4.  0 = "cross" mode: one pass over the pairs between the two row blocks of a

@@ -463,8 +463,8 @@ class DeviceLib:
         return int(self.c.b200_svd_set_fused_max_ld(int(max_ld)))
 
     def svd_set_eig_variant(self, variant):
-        """pivot eigen-solver of the Jacobi rounds: 1 = jacobi_eig_kernel, 3 = jacobi_eig_kernel_v3 (default); other values
-        leave it unchanged; returns the old value"""
+        """pivot eigen-solver of the real Jacobi rounds: 1 = jacobi_eig_kernel<false>, 3 = jacobi_eig_kernel_v3 (default);
+        other values leave it unchanged (complex rounds always use jacobi_eig_kernel<true>); returns the old value"""
         return int(self.c.b200_svd_set_eig_variant(int(variant)))
 
     def block_eigh(self, n, a_off, w_off, v_off, A, W, V):

@@ -15,13 +15,17 @@
 //   A pair whose scaled off-diagonal max |g_ij|/sqrt(g_ii g_jj) is below tol is left untouched; a matrix
 //   is converged once a full cycle of rounds touched nothing.  Singular values = row norms of Y,
 //   sorted on the host (k doubles), vectors written by a final gather kernel.
+// Complex blocks (b200_block_svd_z) run the same driver and the same round kernels instantiated with CPLX = true: Y and
+// W get planar imaginary parts, G = P P^H is Hermitian and the transformation unitary (see jacobi_eig_kernel).
 // Never produces NaN for finite input (the reference falls back gesdd->gesvd for that, npc:4971-4978).
 #include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdlib>
+#include <initializer_list>
 #include <limits>
 #include <numeric>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -61,7 +65,17 @@ struct JMat {
     double amax;                           // max |a_ij| (jacobi_amax_kernel; 0 before it runs)
 };
 
-constexpr int jacobi_smem_bytes() { return 2 * JP * JLDP * (int)sizeof(double); }   // two panel chunks
+// active row blocks for n_act active vectors: an even number (the round-robin pairs the blocks), at least 2, at most nb
+__host__ __device__ inline int j_nb_act(int n_act, int nb) {
+    int nb_act = (n_act + JB - 1) / JB;
+    if (nb_act < 2) nb_act = 2;
+    if (nb_act & 1) ++nb_act;
+    return nb_act > nb ? nb : nb_act;
+}
+
+// dynamic shared memory of the streaming phases: two pipeline stages of one panel chunk per plane
+template <bool CPLX>
+constexpr int jacobi_smem_bytes() { return 2 * (CPLX ? 2 : 1) * JP * JLDP * (int)sizeof(double); }
 
 // Gram diagonals at or below J_GRAM_MIN (Y is the scaled block, max |y| in [1, 2)) are lost in the absolute rounding of
 // subnormal products (~p 2^-1075 per entry): such rows cannot be resolved and are inert, like deflated ones.  Far below
@@ -73,6 +87,31 @@ __device__ __forceinline__ bool j_normal(double x) { return x >= 2.2250738585072
 __device__ __forceinline__ double j_sqrt_prod(double a, double b) {
     const double d = a * b;
     return j_normal(d) ? sqrt(d) : sqrt(a) * sqrt(b);
+}
+
+// max of v over the CTA (JTHREADS threads; red: 32 doubles of shared memory), returned to every thread
+__device__ __forceinline__ double j_cta_max(double v, double *red, int lane, int warp) {
+    v = warp_max(v);
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    v = 0.0;
+#pragma unroll
+    for (int w = 0; w < JTHREADS / 32; ++w) v = fmax(v, red[w]);
+    return v;
+}
+
+// rank of row i of a pivot block (sA: its Gram matrix, stride JLDG) when the rows are ordered by descending diagonal
+// (eigenvalue = norm^2), ties by index.  The key is clamped at 0: the rotated diagonal of a row at rounding level can come
+// out slightly negative and must not sort behind the all-zero padding rows (q..qp-1, always the last positions of a pair),
+// or the padding content (zero Y, W = a unit vector outside the block) would move into a real row
+__device__ __forceinline__ int j_row_rank(const double *sA, int i) {
+    const double di = fmax(sA[i * JLDG + i], 0.0);
+    int rk = 0;
+    for (int k = 0; k < JP; ++k) {
+        const double dk = fmax(sA[k * JLDG + k], 0.0);
+        if (dk > di || (dk == di && k < i)) ++rk;
+    }
+    return rk;
 }
 
 __device__ __forceinline__ void j_load_chunk(double *sP, const double *base, int ld, const int *prow, int col0,
@@ -89,47 +128,64 @@ __device__ __forceinline__ void j_load_chunk(double *sP, const double *base, int
     }
 }
 
-// rows of `base` (ld) <- Q^T rows for the column chunks ch0, ch0+chstep, ... ; prow[0..31] = physical rows
-__device__ __forceinline__ void j_apply(double *bufs, const double (&qa)[2][4][4], double *base, int ld,
-                                        const int *prow, int tid, int ch0, int chstep) {
+// rows of `base` (ld) <- Q^T rows for the column chunks ch0, ch0+chstep, ... ; prow[0..31] = physical rows.
+// q[0] = fragments of Q^T; CPLX: q[1] = those of its imaginary part, basei = the imaginary plane of `base`
+template <bool CPLX>
+__device__ __forceinline__ void j_apply(double *bufs, const double (&q)[CPLX ? 2 : 1][2][4][4], double *base,
+                                        double *basei, int ld, const int *prow, int tid, int ch0, int chstep) {
+    constexpr int STAGE = (CPLX ? 2 : 1) * JP * JLDP;
     const int lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     const int nch = (ld + JKC - 1) / JKC;
     if (ch0 >= nch) return;
     j_load_chunk(bufs, base, ld, prow, ch0 * JKC, tid);
+    if constexpr (CPLX) j_load_chunk(bufs + JP * JLDP, basei, ld, prow, ch0 * JKC, tid);
     cp_async_commit();
     int it = 0;
     for (int ch = ch0; ch < nch; ch += chstep, ++it) {
-        if (ch + chstep < nch) j_load_chunk(bufs + ((it + 1) & 1) * JP * JLDP, base, ld, prow, (ch + chstep) * JKC, tid);
+        if (ch + chstep < nch) {
+            double *nxt = bufs + ((it + 1) & 1) * STAGE;
+            j_load_chunk(nxt, base, ld, prow, (ch + chstep) * JKC, tid);
+            if constexpr (CPLX) j_load_chunk(nxt + JP * JLDP, basei, ld, prow, (ch + chstep) * JKC, tid);
+        }
         cp_async_commit();
         cp_async_wait<1>();
         __syncthreads();
-        const double *sp = bufs + (it & 1) * JP * JLDP;
+        const double *sr = bufs + (it & 1) * STAGE, *si = sr + JP * JLDP;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int nt = warp * 2 + h;
             const int col = ch * JKC + nt * 8;
             if (col < ld) {
-                double acc[2][4];
+                double acc[2][4], acci[2][4];
 #pragma unroll
                 for (int i = 0; i < 2; ++i)
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) acc[i][e] = 0.0;
+                    for (int e = 0; e < 4; ++e) acc[i][e] = acci[i][e] = 0.0;
 #pragma unroll
                 for (int k8 = 0; k8 < 4; ++k8) {
-                    double bf[2];
-                    bf[0] = sp[(k8 * 8 + t) * JLDP + nt * 8 + g];
-                    bf[1] = sp[(k8 * 8 + t + 4) * JLDP + nt * 8 + g];
-                    dmma_16x8x8(acc[0], qa[0][k8], bf);
-                    dmma_16x8x8(acc[1], qa[1][k8], bf);
+                    const int b0 = (k8 * 8 + t) * JLDP + nt * 8 + g, b1 = (k8 * 8 + t + 4) * JLDP + nt * 8 + g;
+                    double br[2] = {sr[b0], sr[b1]};
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        dmma_16x8x8(acc[i], q[0][i][k8], br);
+                        if constexpr (CPLX) {   // Re += -Qi Pi,  Im += Qr Pi + Qi Pr
+                            const double(&qi)[4] = q[1][i][k8];
+                            double nqi[4] = {-qi[0], -qi[1], -qi[2], -qi[3]};
+                            double bi[2] = {si[b0], si[b1]};
+                            dmma_16x8x8(acc[i], nqi, bi);
+                            dmma_16x8x8(acci[i], q[0][i][k8], bi);
+                            dmma_16x8x8(acci[i], qi, br);
+                        }
+                    }
                 }
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
 #pragma unroll
                     for (int hh = 0; hh < 2; ++hh) {
-                        int pr = i * 16 + g + 8 * hh;
-                        int grow = prow[pr];
-                        double *dst = base + (int64_t)grow * ld + col + 2 * t;
-                        *reinterpret_cast<double2 *>(dst) = make_double2(acc[i][2 * hh], acc[i][2 * hh + 1]);
+                        const int64_t o = (int64_t)prow[i * 16 + g + 8 * hh] * ld + col + 2 * t;
+                        *reinterpret_cast<double2 *>(base + o) = make_double2(acc[i][2 * hh], acc[i][2 * hh + 1]);
+                        if constexpr (CPLX)
+                            *reinterpret_cast<double2 *>(basei + o) = make_double2(acci[i][2 * hh], acci[i][2 * hh + 1]);
                     }
                 }
             }
@@ -167,15 +223,20 @@ __device__ __forceinline__ bool j_pair_rows(const JMat &mt, int j, int round, co
 // One Jacobi round = three launches, so that the streaming phases use the whole GPU:
 //   jacobi_gram_kernel  grid (nsplit, pairs): partial G = P P^T over a subset of the column chunks (DMMA),
 //                       one 32x32 partial per split in Gbuf[pair][split]
-//   jacobi_eig_kernel   grid (pairs): convergence test, parallel cyclic Jacobi on G in shared memory, Q^T (rows
-//                       ordered by descending eigenvalue) -> QTbuf[pair], flag[pair] = rotated
+//   jacobi_eig_kernel   grid (pairs): convergence test, parallel cyclic Jacobi on G, Q^T (rows ordered by descending
+//   (or _v3)            eigenvalue) -> QTbuf[pair], flag[pair] = rotated
 //   jacobi_apply_kernel grid (nsplit, pairs, 2): P <- Q^T P (z = 0) and the same rows of W <- Q^T W (z = 1)
+// CPLX = true (complex blocks): every streamed chunk has a real and an imaginary plane, each phase is four real DMMA
+// products (Re G = Pr Pr^T + Pi Pi^T, Im G = Pi Pr^T - Pr Pi^T;  Re P' = Tr Pr - Ti Pi, Im P' = Tr Pi + Ti Pr), and the Gram
+// partials and Q^T (= T) are stored as [real 32x32 | imaginary 32x32] per pair (and split).
 // (the three phases are device functions so that jacobi_round_fused_kernel can run them back to back in one launch; buffers
 // one phase writes and the next one reads -- Gbuf, QTbuf, flags, work -- are deliberately NOT const __restrict__ there: the
 // read-only data path is not coherent with writes of the same kernel)
+template <bool CPLX>
 __device__ __forceinline__ void jacobi_gram_body(double *bufs, const double *work, const JMat *__restrict__ mats,
                                                  const int *__restrict__ cta_mat, const int *__restrict__ rmap, int round,
                                                  const int *__restrict__ done, double *Gbuf, int split, int nsplit, int pair) {
+    constexpr int NPL = CPLX ? 2 : 1, STAGE = NPL * JP * JLDP;
     __shared__ int s_rows[JP];
     const int mi = cta_mat[pair];
     if (done[mi]) return;
@@ -183,64 +244,85 @@ __device__ __forceinline__ void jacobi_gram_body(double *bufs, const double *wor
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
     if (!j_pair_rows(mt, pair - mt.cta_begin, round, rmap, s_rows, tid)) return;
     __syncthreads();
-    const double *Y = work + mt.y_off;
+    const double *Y = work + mt.y_off, *Yi = work + mt.yi_off;
     const int ld = mt.ldy;
     const int nch = (ld + JKC - 1) / JKC;
     const int ch0 = split, chstep = nsplit;
     if (ch0 >= nch) return;
     const int tm = warp >> 2, tn = warp & 3;  // 2 x 4 tiles of 16 x 8
-    double acc[4] = {0.0, 0.0, 0.0, 0.0};
+    double acc[4] = {0.0, 0.0, 0.0, 0.0}, acci[4] = {0.0, 0.0, 0.0, 0.0};
     j_load_chunk(bufs, Y, ld, s_rows, ch0 * JKC, tid);
+    if constexpr (CPLX) j_load_chunk(bufs + JP * JLDP, Yi, ld, s_rows, ch0 * JKC, tid);
     cp_async_commit();
     int it = 0;
     for (int ch = ch0; ch < nch; ch += chstep, ++it) {
-        if (ch + chstep < nch) j_load_chunk(bufs + ((it + 1) & 1) * JP * JLDP, Y, ld, s_rows, (ch + chstep) * JKC, tid);
+        if (ch + chstep < nch) {
+            double *nxt = bufs + ((it + 1) & 1) * STAGE;
+            j_load_chunk(nxt, Y, ld, s_rows, (ch + chstep) * JKC, tid);
+            if constexpr (CPLX) j_load_chunk(nxt + JP * JLDP, Yi, ld, s_rows, (ch + chstep) * JKC, tid);
+        }
         cp_async_commit();
         cp_async_wait<1>();
         __syncthreads();
-        const double *sp = bufs + (it & 1) * JP * JLDP;
-#pragma unroll
+        const double *sr = bufs + (it & 1) * STAGE, *si = sr + JP * JLDP;
+#pragma unroll (CPLX ? 4 : JKC / 8)
         for (int k8 = 0; k8 < JKC / 8; ++k8) {
-            double af[4], bf[2];
-            const double *ap = sp + (tm * 16 + g) * JLDP + k8 * 8 + t;
-            af[0] = ap[0];
-            af[1] = ap[8 * JLDP];
-            af[2] = ap[4];
-            af[3] = ap[8 * JLDP + 4];
-            const double *bp = sp + (tn * 8 + g) * JLDP + k8 * 8 + t;
-            bf[0] = bp[0];
-            bf[1] = bp[4];
-            dmma_16x8x8(acc, af, bf);
+            const int ao = (tm * 16 + g) * JLDP + k8 * 8 + t, bo = (tn * 8 + g) * JLDP + k8 * 8 + t;
+            double ar[4] = {sr[ao], sr[ao + 8 * JLDP], sr[ao + 4], sr[ao + 8 * JLDP + 4]};
+            double br[2] = {sr[bo], sr[bo + 4]};
+            dmma_16x8x8(acc, ar, br);
+            if constexpr (CPLX) {   // Re G += Pi Pi^T,  Im G += Pi Pr^T - Pr Pi^T
+                double ai[4] = {si[ao], si[ao + 8 * JLDP], si[ao + 4], si[ao + 8 * JLDP + 4]};
+                double nar[4] = {-ar[0], -ar[1], -ar[2], -ar[3]};
+                double bi[2] = {si[bo], si[bo + 4]};
+                dmma_16x8x8(acc, ai, bi);
+                dmma_16x8x8(acci, ai, br);
+                dmma_16x8x8(acci, nar, bi);
+            }
         }
         __syncthreads();
     }
     cp_async_wait<0>();
     // partial result of this column split (summed in a fixed order by the eigen-solver phase: deterministic)
-    double *G = Gbuf + ((int64_t)pair * nsplit + split) * (JP * JP);
+    double *G = Gbuf + ((int64_t)pair * nsplit + split) * (NPL * JP * JP);
     const int r0 = tm * 16 + g, c0 = tn * 8 + 2 * t;
-    G[r0 * JP + c0] = acc[0];
-    G[r0 * JP + c0 + 1] = acc[1];
-    G[(r0 + 8) * JP + c0] = acc[2];
-    G[(r0 + 8) * JP + c0 + 1] = acc[3];
+#pragma unroll
+    for (int part = 0; part < NPL; ++part) {
+        const double *a = part ? acci : acc;
+        double *Gp = G + part * (JP * JP);
+        Gp[r0 * JP + c0] = a[0];
+        Gp[r0 * JP + c0 + 1] = a[1];
+        Gp[(r0 + 8) * JP + c0] = a[2];
+        Gp[(r0 + 8) * JP + c0 + 1] = a[3];
+    }
 }
 
+template <bool CPLX>
 __global__ void __launch_bounds__(JTHREADS)
     jacobi_gram_kernel(const double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ cta_mat,
                        const int *__restrict__ rmap, int round, const int *__restrict__ done,
                        double *__restrict__ Gbuf) {
     extern __shared__ __align__(16) double jsmem[];
-    jacobi_gram_body(jsmem, work, mats, cta_mat, rmap, round, done, Gbuf, blockIdx.x, gridDim.x, blockIdx.y);
+    jacobi_gram_body<CPLX>(jsmem, work, mats, cta_mat, rmap, round, done, Gbuf, blockIdx.x, gridDim.x, blockIdx.y);
 }
 
+// Pivot solver 1, real (CPLX = false) and complex: grid (pairs), G and T in shared memory.  Convergence test, then T with
+// T G T^H diagonal by parallel cyclic Jacobi (16 disjoint pairs per rotation set, round-robin order), rows of T ordered by
+// descending eigenvalue -> QTbuf[pair], flag[pair] = rotated.  The rotation of the pair (p, q) is the real rotation (c, s)
+// of (g_pp, g_qq, |g_pq|) after the phase e = g_pq / |g_pq| of a complex g_pq is stripped (e = 1 for real blocks):
+//   rows of G and T:  row p <- c x_p - s e x_q,  row q <- s x_p + c e x_q
+//   columns of G:     col p <- c y_p - s conj(e) y_q,  col q <- s y_p + c conj(e) y_q
+template <bool CPLX>
 __global__ void __launch_bounds__(JTHREADS)
     jacobi_eig_kernel(const JMat *__restrict__ mats, const int *__restrict__ cta_mat, int *__restrict__ rot_count,
                       const int *__restrict__ done, double tol_scale, const double *__restrict__ Gbuf, int nsplit,
-                      double *__restrict__ QTbuf, int *__restrict__ flags) {
-    __shared__ double sG[JP * JLDG];
-    __shared__ double sQ[JP * JLDG];
-    __shared__ double cs_c[JB], cs_s[JB];
+                      double *__restrict__ QTbuf, int *__restrict__ flags, int inner_sweeps) {
+    constexpr int NPL = CPLX ? 2 : 1;
+    __shared__ double sG[NPL][JP * JLDG], sT[NPL][JP * JLDG];   // [real | imaginary]
+    __shared__ double cs_c[JB], cs_s[JB], cs_er[JB], cs_ei[JB];
     __shared__ int pr_p[JB], pr_q[JB];
     __shared__ double red[32];
+    __shared__ int s_rank[JP];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (tid == 0) flags[blockIdx.x] = 0;
     const int mi = cta_mat[blockIdx.x];
@@ -250,51 +332,43 @@ __global__ void __launch_bounds__(JTHREADS)
     {
         const int nch = (mt.ldy + JKC - 1) / JKC;
         const int ns = nsplit < nch ? nsplit : nch;
-        const double *G = Gbuf + (int64_t)blockIdx.x * nsplit * (JP * JP);
+        const double *G = Gbuf + (int64_t)blockIdx.x * nsplit * (NPL * JP * JP);
         for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
-            double v = 0.0;
-            for (int sp = 0; sp < ns; ++sp) v += G[sp * (JP * JP) + idx];
-            sG[(idx / JP) * JLDG + (idx % JP)] = v;
+            const int r = idx / JP, c = idx % JP;
+#pragma unroll
+            for (int pl = 0; pl < NPL; ++pl) {
+                double v = 0.0;
+                for (int sp = 0; sp < ns; ++sp) v += G[sp * (NPL * JP * JP) + pl * (JP * JP) + idx];
+                sG[pl][r * JLDG + c] = v;
+                sT[pl][r * JLDG + c] = (pl == 0 && r == c) ? 1.0 : 0.0;
+            }
         }
     }
     __syncthreads();
 
-    // ---- convergence measure of this pair ----
+    // ---- convergence measure of this pair: max |g_rc| / sqrt(g_rr g_cc) over the non-negligible rows ----
+    // (square roots taken separately where g_rr g_cc over- or underflows: blocks scaled near 1e+-150)
     const double defl2 = fmax(mt.defl * mt.defl, J_GRAM_MIN);
     double offmax = 0.0;
     for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
-        int r = idx / JP, c = idx % JP;
+        const int r = idx / JP, c = idx % JP;
         if (r < c) {
-            const double drr = sG[r * JLDG + r], dcc = sG[c * JLDG + c];
-            double o = fabs(sG[r * JLDG + c]);
+            const double drr = sG[0][r * JLDG + r], dcc = sG[0][c * JLDG + c];
             if (drr > defl2 && dcc > defl2) {   // negligible (deflated) rows are inert
-                double v = o / j_sqrt_prod(drr, dcc);
-                offmax = fmax(offmax, v);
+                if constexpr (CPLX)
+                    offmax = fmax(offmax, hypot(sG[0][r * JLDG + c], sG[1][r * JLDG + c]) / (sqrt(drr) * sqrt(dcc)));
+                else
+                    offmax = fmax(offmax, fabs(sG[0][r * JLDG + c]) / j_sqrt_prod(drr, dcc));
             }
         }
     }
-    offmax = warp_max(offmax);
-    if (lane == 0) red[warp] = offmax;
-    __syncthreads();
-    if (tid == 0) {
-        double v = 0.0;
-        for (int w = 0; w < JTHREADS / 32; ++w) v = fmax(v, red[w]);
-        red[0] = v;
-    }
-    __syncthreads();
-    offmax = red[0];
+    offmax = j_cta_max(offmax, red, lane, warp);
     const double tol = tol_scale * sqrt((double)mt.p);
     if (!(offmax > tol)) return;  // uniform for the whole CTA
     if (tid == 0) atomicAdd(&rot_count[mi], 1);
 
-    // ---- phase 2: G = Q L Q^T by parallel cyclic Jacobi ----
-    for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
-        int r = idx / JP, c = idx % JP;
-        sQ[r * JLDG + c] = (r == c) ? 1.0 : 0.0;
-    }
-    __syncthreads();
     const double tol_in = 1e-15;
-    for (int sweep = 0; sweep < J_INNER_SWEEPS; ++sweep) {
+    for (int sweep = 0; sweep < inner_sweeps; ++sweep) {
         int any = 0;
         for (int step = 0; step < JP - 1; ++step) {
             if (tid < JB) {
@@ -306,69 +380,98 @@ __global__ void __launch_bounds__(JTHREADS)
                     a = (step + tid) % (JP - 1);
                     b = (step - tid + (JP - 1)) % (JP - 1);
                 }
-                int p = a < b ? a : b, q = a < b ? b : a;
-                double gpp = sG[p * JLDG + p], gqq = sG[q * JLDG + q], gpq = sG[p * JLDG + q];
-                double c = 1.0, s = 0.0;
-                double lim = tol_in * j_sqrt_prod(fabs(gpp), fabs(gqq));
-                if (fabs(gpq) > lim && gpp > defl2 && gqq > defl2) {
-                    // t = tan(theta) of the Jacobi rotation: one sqrt, one division, one rsqrt (hypot where aa^2 + bb^2
-                    // is not a normal number)
-                    const double aa = gqq - gpp, bb = 2.0 * gpq;
-                    const double h2 = aa * aa + bb * bb;
-                    const double hh = j_normal(h2) ? sqrt(h2) : hypot(aa, bb);
-                    const double tt = (aa >= 0.0) ? bb / (aa + hh) : bb / (aa - hh);
-                    c = rsqrt(1.0 + tt * tt);
-                    s = tt * c;
-                    any = 1;
+                const int p = a < b ? a : b, q = a < b ? b : a;
+                const double gpp = sG[0][p * JLDG + p], gqq = sG[0][q * JLDG + q], gpq = sG[0][p * JLDG + q];
+                double c = 1.0, s = 0.0, er = 1.0, ei = 0.0;
+                // t = tan(theta) of the Jacobi rotation: one sqrt or hypot, one division, one rsqrt
+                if constexpr (CPLX) {
+                    const double gi = sG[1][p * JLDG + q], ag = hypot(gpq, gi);
+                    if (gpp > defl2 && gqq > defl2 && ag > tol_in * sqrt(gpp) * sqrt(gqq)) {
+                        er = gpq / ag;
+                        ei = gi / ag;
+                        const double aa = gqq - gpp, bb = 2.0 * ag;
+                        const double hh = hypot(aa, bb);
+                        const double tt = (aa >= 0.0) ? bb / (aa + hh) : bb / (aa - hh);
+                        c = rsqrt(1.0 + tt * tt);
+                        s = tt * c;
+                        any = 1;
+                    }
+                } else {   // (hypot only where aa^2 + bb^2 is not a normal number)
+                    const double lim = tol_in * j_sqrt_prod(fabs(gpp), fabs(gqq));
+                    if (fabs(gpq) > lim && gpp > defl2 && gqq > defl2) {
+                        const double aa = gqq - gpp, bb = 2.0 * gpq;
+                        const double h2 = aa * aa + bb * bb;
+                        const double hh = j_normal(h2) ? sqrt(h2) : hypot(aa, bb);
+                        const double tt = (aa >= 0.0) ? bb / (aa + hh) : bb / (aa - hh);
+                        c = rsqrt(1.0 + tt * tt);
+                        s = tt * c;
+                        any = 1;
+                    }
                 }
                 pr_p[tid] = p;
                 pr_q[tid] = q;
                 cs_c[tid] = c;
                 cs_s[tid] = s;
+                if constexpr (CPLX) {
+                    cs_er[tid] = er;
+                    cs_ei[tid] = ei;
+                }
             }
             __syncthreads();
-            for (int idx = tid; idx < JB * JP; idx += JTHREADS) {  // rows
-                int jj = idx / JP, col = idx % JP;
-                int p = pr_p[jj], q = pr_q[jj];
-                double c = cs_c[jj], s = cs_s[jj];
-                double gp = sG[p * JLDG + col], gq = sG[q * JLDG + col];
-                sG[p * JLDG + col] = c * gp - s * gq;
-                sG[q * JLDG + col] = s * gp + c * gq;
+            // rows of G and T:  row p <- c x_p - s y,  row q <- s x_p + c y,  y = e x_q
+            for (int idx = tid; idx < JB * JP; idx += JTHREADS) {
+                const int jj = idx / JP, col = idx % JP;
+                const int p = pr_p[jj], q = pr_q[jj];
+                const double c = cs_c[jj], s = cs_s[jj];
+#pragma unroll
+                for (int which = 0; which < 2; ++which) {
+                    double *Xr = which ? sT[0] : sG[0];
+                    const double xpr = Xr[p * JLDG + col];
+                    double yr = Xr[q * JLDG + col];
+                    if constexpr (CPLX) {
+                        double *Xi = which ? sT[1] : sG[1];
+                        const double er = cs_er[jj], ei = cs_ei[jj];
+                        const double xpi = Xi[p * JLDG + col], xqr = yr, xqi = Xi[q * JLDG + col];
+                        yr = er * xqr - ei * xqi;
+                        const double yi = er * xqi + ei * xqr;
+                        Xi[p * JLDG + col] = c * xpi - s * yi;
+                        Xi[q * JLDG + col] = s * xpi + c * yi;
+                    }
+                    Xr[p * JLDG + col] = c * xpr - s * yr;
+                    Xr[q * JLDG + col] = s * xpr + c * yr;
+                }
             }
             __syncthreads();
-            for (int idx = tid; idx < JB * JP; idx += JTHREADS) {  // columns of G and Q
-                int jj = idx / JP, row = idx % JP;
-                int p = pr_p[jj], q = pr_q[jj];
-                double c = cs_c[jj], s = cs_s[jj];
-                double gp = sG[row * JLDG + p], gq = sG[row * JLDG + q];
-                sG[row * JLDG + p] = c * gp - s * gq;
-                sG[row * JLDG + q] = s * gp + c * gq;
-                double qp_ = sQ[row * JLDG + p], qq_ = sQ[row * JLDG + q];
-                sQ[row * JLDG + p] = c * qp_ - s * qq_;
-                sQ[row * JLDG + q] = s * qp_ + c * qq_;
+            // columns of G (G <- G T^H):  col p <- c y_p - s z,  col q <- s y_p + c z,  z = conj(e) y_q
+            for (int idx = tid; idx < JB * JP; idx += JTHREADS) {
+                const int jj = idx / JP, row = idx % JP;
+                const int p = pr_p[jj], q = pr_q[jj];
+                const double c = cs_c[jj], s = cs_s[jj];
+                const double ypr = sG[0][row * JLDG + p];
+                double zr = sG[0][row * JLDG + q];
+                if constexpr (CPLX) {
+                    const double er = cs_er[jj], ei = cs_ei[jj];
+                    const double ypi = sG[1][row * JLDG + p], yqr = zr, yqi = sG[1][row * JLDG + q];
+                    zr = er * yqr + ei * yqi;
+                    const double zi = er * yqi - ei * yqr;
+                    sG[1][row * JLDG + p] = c * ypi - s * zi;
+                    sG[1][row * JLDG + q] = s * ypi + c * zi;
+                }
+                sG[0][row * JLDG + p] = c * ypr - s * zr;
+                sG[0][row * JLDG + q] = s * ypr + c * zr;
             }
             __syncthreads();
         }
         if (!__syncthreads_or(any)) break;
     }
-    // order the new rows by descending eigenvalue (norm^2): helps the outer convergence (de Rijk)
-    // rank[i] = number of entries with larger diagonal (ties by index); the key is clamped at 0 (see zjacobi_eig_kernel)
-    if (tid < JP) {
-        double di = fmax(sG[tid * JLDG + tid], 0.0);
-        int rk = 0;
-        for (int k = 0; k < JP; ++k) {
-            double dk = fmax(sG[k * JLDG + k], 0.0);
-            if (dk > di || (dk == di && k < tid)) ++rk;
-        }
-        // store rank in sG's unused padding column
-        sG[tid * JLDG + JP] = (double)rk;
-    }
+    // rows of T ordered by descending eigenvalue (norm^2): helps the outer convergence (de Rijk)
+    if (tid < JP) s_rank[tid] = j_row_rank(sG[0], tid);
     __syncthreads();
-    double *QT = QTbuf + (int64_t)blockIdx.x * (JP * JP);
+    double *QT = QTbuf + (int64_t)blockIdx.x * (NPL * JP * JP);
     for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
-        int i = idx / JP, k = idx % JP;
-        int rk = (int)sG[i * JLDG + JP];
-        QT[rk * JP + k] = sQ[k * JLDG + i];
+        const int i = idx / JP, k = idx % JP;
+#pragma unroll
+        for (int pl = 0; pl < NPL; ++pl) QT[pl * (JP * JP) + s_rank[i] * JP + k] = sT[pl][i * JLDG + k];
     }
     if (tid == 0) flags[blockIdx.x] = 1;
 }
@@ -478,12 +581,7 @@ __device__ __forceinline__ void jacobi_eig_v3_body(const JMat *__restrict__ mats
             if (lane < c && dl > defl2 && dc > defl2) offmax = fmax(offmax, fabs(g[i]) / j_sqrt_prod(dl, dc));
         }
     }
-    offmax = warp_max(offmax);
-    if (lane == 0) red[warp] = offmax;
-    __syncthreads();
-    offmax = 0.0;
-#pragma unroll
-    for (int w = 0; w < JTHREADS / 32; ++w) offmax = fmax(offmax, red[w]);
+    offmax = j_cta_max(offmax, red, lane, warp);
     const double tol = tol_scale * sqrt((double)mt.p);
     if (!(offmax > tol)) return;  // uniform for the whole CTA
     if (tid == 0) atomicAdd(&rot_count[mi], 1);
@@ -545,17 +643,8 @@ __device__ __forceinline__ void jacobi_eig_v3_body(const JMat *__restrict__ mats
         if (tid == 0) s_any = 0;
         __syncthreads();
     }
-    // order the new rows by descending eigenvalue (norm^2): rank[i] = number of entries with larger diagonal (ties by index);
-    // the key is clamped at 0, as in zjacobi_eig_kernel: a rank-deficient block must not lose a row to a padding row
-    if (tid < JP) {
-        const double di = fmax(sA[tid * JLDG + tid], 0.0);
-        int rk = 0;
-        for (int k = 0; k < JP; ++k) {
-            const double dk = fmax(sA[k * JLDG + k], 0.0);
-            if (dk > di || (dk == di && k < tid)) ++rk;
-        }
-        s_rank[tid] = rk;
-    }
+    // order the new rows by descending eigenvalue (norm^2)
+    if (tid < JP) s_rank[tid] = j_row_rank(sA, tid);
     __syncthreads();
     double *QT = QTbuf + (int64_t)pair * (JP * JP);
     // QT[rank[i]][k] = Q[k][i]; this thread holds Q[4w+j][lane]
@@ -571,10 +660,12 @@ __global__ void __launch_bounds__(JTHREADS)
     jacobi_eig_v3_body(mats, cta_mat, rot_count, done, tol_scale, Gbuf, nsplit, QTbuf, flags, inner_sweeps, round, blockIdx.x);
 }
 
+template <bool CPLX>
 __device__ __forceinline__ void jacobi_apply_body(double *bufs, double *work, const JMat *__restrict__ mats,
                                                   const int *__restrict__ cta_mat, const int *__restrict__ rmap, int round,
                                                   const double *QTbuf, const int *flags, int split, int nsplit, int pair,
                                                   int which) {
+    constexpr int NPL = CPLX ? 2 : 1;
     __shared__ int s_rows[JP];
     if (!flags[pair]) return;
     const int mi = cta_mat[pair];
@@ -582,30 +673,34 @@ __device__ __forceinline__ void jacobi_apply_body(double *bufs, double *work, co
     const int tid = threadIdx.x, lane = tid & 31, g = lane >> 2, t = lane & 3;
     if (!j_pair_rows(mt, pair - mt.cta_begin, round, rmap, s_rows, tid)) return;
     __syncthreads();
-    const double *QT = QTbuf + (int64_t)pair * (JP * JP);
-    double qa[2][4][4];
+    const double *QT = QTbuf + (int64_t)pair * (NPL * JP * JP);
+    double qa[NPL][2][4][4];
 #pragma unroll
-    for (int i = 0; i < 2; ++i)
+    for (int pl = 0; pl < NPL; ++pl)
 #pragma unroll
-        for (int k8 = 0; k8 < 4; ++k8) {
-            const double *ap = QT + (i * 16 + g) * JP + k8 * 8 + t;
-            qa[i][k8][0] = ap[0];
-            qa[i][k8][1] = ap[8 * JP];
-            qa[i][k8][2] = ap[4];
-            qa[i][k8][3] = ap[8 * JP + 4];
-        }
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+            for (int k8 = 0; k8 < 4; ++k8) {
+                const double *ap = QT + pl * (JP * JP) + (i * 16 + g) * JP + k8 * 8 + t;
+                qa[pl][i][k8][0] = ap[0];
+                qa[pl][i][k8][1] = ap[8 * JP];
+                qa[pl][i][k8][2] = ap[4];
+                qa[pl][i][k8][3] = ap[8 * JP + 4];
+            }
     if (which == 0)
-        j_apply(bufs, qa, work + mt.y_off, mt.ldy, s_rows, tid, split, nsplit);
+        j_apply<CPLX>(bufs, qa, work + mt.y_off, work + mt.yi_off, mt.ldy, s_rows, tid, split, nsplit);
     else
-        j_apply(bufs, qa, work + mt.w_off, mt.ldw, s_rows, tid, split, nsplit);
+        j_apply<CPLX>(bufs, qa, work + mt.w_off, work + mt.wi_off, mt.ldw, s_rows, tid, split, nsplit);
 }
 
+template <bool CPLX>
 __global__ void __launch_bounds__(JTHREADS)
     jacobi_apply_kernel(double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ cta_mat,
                         const int *__restrict__ rmap, int round, const double *__restrict__ QTbuf,
                         const int *__restrict__ flags) {
     extern __shared__ __align__(16) double jsmem[];
-    jacobi_apply_body(jsmem, work, mats, cta_mat, rmap, round, QTbuf, flags, blockIdx.x, gridDim.x, blockIdx.y, blockIdx.z);
+    jacobi_apply_body<CPLX>(jsmem, work, mats, cta_mat, rmap, round, QTbuf, flags, blockIdx.x, gridDim.x, blockIdx.y,
+                            blockIdx.z);
 }
 
 // Small-block regime: one launch per round.  For matrices of a few hundred columns the three phases of a pair are a few
@@ -618,321 +713,13 @@ __global__ void __launch_bounds__(JTHREADS)
                               double tol_scale, double *Gbuf, double *QTbuf, int *flags, int inner_sweeps) {
     extern __shared__ __align__(16) double jsmem[];
     const int pair = blockIdx.x;
-    jacobi_gram_body(jsmem, work, mats, cta_mat, rmap, round, done, Gbuf, 0, 1, pair);
+    jacobi_gram_body<false>(jsmem, work, mats, cta_mat, rmap, round, done, Gbuf, 0, 1, pair);
     __syncthreads();
     jacobi_eig_v3_body(mats, cta_mat, rot_count, done, tol_scale, Gbuf, 1, QTbuf, flags, inner_sweeps, round, pair);
     __syncthreads();
-    jacobi_apply_body(jsmem, work, mats, cta_mat, rmap, round, QTbuf, flags, 0, 1, pair, 0);
+    jacobi_apply_body<false>(jsmem, work, mats, cta_mat, rmap, round, QTbuf, flags, 0, 1, pair, 0);
     __syncthreads();
-    jacobi_apply_body(jsmem, work, mats, cta_mat, rmap, round, QTbuf, flags, 0, 1, pair, 1);
-}
-
-// ---- complex one-sided Jacobi (b200_block_svd_z) ---------------------------------------------------
-// Planar data: Y = Yr + i Yi, W = Wr + i Wi.  The same rounds, pairs, convergence test and deflation as the real path;
-// only the arithmetic of the three phases differs:
-//   zjacobi_gram_kernel   G = P P^H:  Re G = Pr Pr^T + Pi Pi^T,  Im G = Pi Pr^T - Pr Pi^T  (four real DMMA products)
-//   zjacobi_eig_kernel    unitary T with T G T^H diagonal by cyclic complex Jacobi rotations: for the pair (p, q) the phase
-//                         e = g_pq / |g_pq| is stripped (row q <- e row q makes g_pq real), then the real rotation of
-//                         (g_pp, g_qq, |g_pq|):  row p <- c x_p - s e x_q,  row q <- s x_p + c e x_q
-//   zjacobi_apply_kernel  P <- T P and W <- T W:  Re = Tr Pr - Ti Pi,  Im = Tr Pi + Ti Pr  (four real DMMA products)
-// Gram partials and T are stored as [real 32x32 | imaginary 32x32] per pair (and split).
-constexpr int ZJ_STAGE = 2 * JP * JLDP;   // doubles of one pipeline stage: real chunk, imaginary chunk
-constexpr int zjacobi_smem_bytes() { return 2 * ZJ_STAGE * (int)sizeof(double); }
-
-__global__ void __launch_bounds__(JTHREADS)
-    zjacobi_gram_kernel(const double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ cta_mat,
-                        const int *__restrict__ rmap, int round, const int *__restrict__ done, double *__restrict__ Gbuf) {
-    extern __shared__ __align__(16) double jsmem[];
-    __shared__ int s_rows[JP];
-    const int split = blockIdx.x, nsplit = gridDim.x, pair = blockIdx.y;
-    const int mi = cta_mat[pair];
-    if (done[mi]) return;
-    const JMat mt = mats[mi];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
-    if (!j_pair_rows(mt, pair - mt.cta_begin, round, rmap, s_rows, tid)) return;
-    __syncthreads();
-    const double *Yr = work + mt.y_off, *Yi = work + mt.yi_off;
-    const int ld = mt.ldy;
-    const int nch = (ld + JKC - 1) / JKC;
-    if (split >= nch) return;
-    const int tm = warp >> 2, tn = warp & 3;  // 2 x 4 tiles of 16 x 8
-    double accr[4] = {0.0, 0.0, 0.0, 0.0}, acci[4] = {0.0, 0.0, 0.0, 0.0};
-    j_load_chunk(jsmem, Yr, ld, s_rows, split * JKC, tid);
-    j_load_chunk(jsmem + JP * JLDP, Yi, ld, s_rows, split * JKC, tid);
-    cp_async_commit();
-    int it = 0;
-    for (int ch = split; ch < nch; ch += nsplit, ++it) {
-        if (ch + nsplit < nch) {
-            double *nxt = jsmem + ((it + 1) & 1) * ZJ_STAGE;
-            j_load_chunk(nxt, Yr, ld, s_rows, (ch + nsplit) * JKC, tid);
-            j_load_chunk(nxt + JP * JLDP, Yi, ld, s_rows, (ch + nsplit) * JKC, tid);
-        }
-        cp_async_commit();
-        cp_async_wait<1>();
-        __syncthreads();
-        const double *sr = jsmem + (it & 1) * ZJ_STAGE, *si = sr + JP * JLDP;
-#pragma unroll 4
-        for (int k8 = 0; k8 < JKC / 8; ++k8) {
-            const int ao = (tm * 16 + g) * JLDP + k8 * 8 + t, bo = (tn * 8 + g) * JLDP + k8 * 8 + t;
-            double ar[4] = {sr[ao], sr[ao + 8 * JLDP], sr[ao + 4], sr[ao + 8 * JLDP + 4]};
-            double ai[4] = {si[ao], si[ao + 8 * JLDP], si[ao + 4], si[ao + 8 * JLDP + 4]};
-            double nar[4] = {-ar[0], -ar[1], -ar[2], -ar[3]};
-            double br[2] = {sr[bo], sr[bo + 4]}, bi[2] = {si[bo], si[bo + 4]};
-            dmma_16x8x8(accr, ar, br);
-            dmma_16x8x8(accr, ai, bi);
-            dmma_16x8x8(acci, ai, br);
-            dmma_16x8x8(acci, nar, bi);
-        }
-        __syncthreads();
-    }
-    cp_async_wait<0>();
-    double *G = Gbuf + ((int64_t)pair * nsplit + split) * (2 * JP * JP);
-    const int r0 = tm * 16 + g, c0 = tn * 8 + 2 * t;
-#pragma unroll
-    for (int part = 0; part < 2; ++part) {
-        const double *acc = part ? acci : accr;
-        double *Gp = G + part * (JP * JP);
-        Gp[r0 * JP + c0] = acc[0];
-        Gp[r0 * JP + c0 + 1] = acc[1];
-        Gp[(r0 + 8) * JP + c0] = acc[2];
-        Gp[(r0 + 8) * JP + c0 + 1] = acc[3];
-    }
-}
-
-__global__ void __launch_bounds__(JTHREADS)
-    zjacobi_eig_kernel(const JMat *__restrict__ mats, const int *__restrict__ cta_mat, int *__restrict__ rot_count,
-                       const int *__restrict__ done, double tol_scale, const double *__restrict__ Gbuf, int nsplit,
-                       double *__restrict__ QTbuf, int *__restrict__ flags, int inner_sweeps) {
-    __shared__ double sGr[JP * JLDG], sGi[JP * JLDG], sTr[JP * JLDG], sTi[JP * JLDG];
-    __shared__ double cs_c[JB], cs_s[JB], cs_er[JB], cs_ei[JB];
-    __shared__ int pr_p[JB], pr_q[JB];
-    __shared__ double red[32];
-    __shared__ int s_rank[JP];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) flags[blockIdx.x] = 0;
-    const int mi = cta_mat[blockIdx.x];
-    if (done[mi]) return;
-    const JMat mt = mats[mi];
-    if (2 * (blockIdx.x - mt.cta_begin) >= mt.nb_act) return;
-    {
-        const int nch = (mt.ldy + JKC - 1) / JKC;
-        const int ns = nsplit < nch ? nsplit : nch;
-        const double *G = Gbuf + (int64_t)blockIdx.x * nsplit * (2 * JP * JP);
-        for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
-            double vr = 0.0, vi = 0.0;
-            for (int sp = 0; sp < ns; ++sp) {
-                vr += G[sp * (2 * JP * JP) + idx];
-                vi += G[sp * (2 * JP * JP) + JP * JP + idx];
-            }
-            const int r = idx / JP, c = idx % JP;
-            sGr[r * JLDG + c] = vr;
-            sGi[r * JLDG + c] = vi;
-            sTr[r * JLDG + c] = (r == c) ? 1.0 : 0.0;
-            sTi[r * JLDG + c] = 0.0;
-        }
-    }
-    __syncthreads();
-
-    // ---- convergence measure of this pair: max |g_rc| / sqrt(g_rr g_cc) over the non-negligible rows ----
-    // (square roots taken separately and hypot below: g_rr g_cc over- or underflows for blocks scaled near 1e+-150)
-    const double defl2 = fmax(mt.defl * mt.defl, J_GRAM_MIN);
-    double offmax = 0.0;
-    for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
-        const int r = idx / JP, c = idx % JP;
-        if (r < c) {
-            const double drr = sGr[r * JLDG + r], dcc = sGr[c * JLDG + c];
-            if (drr > defl2 && dcc > defl2)
-                offmax = fmax(offmax, hypot(sGr[r * JLDG + c], sGi[r * JLDG + c]) / (sqrt(drr) * sqrt(dcc)));
-        }
-    }
-    offmax = warp_max(offmax);
-    if (lane == 0) red[warp] = offmax;
-    __syncthreads();
-    offmax = 0.0;
-#pragma unroll
-    for (int w = 0; w < JTHREADS / 32; ++w) offmax = fmax(offmax, red[w]);
-    const double tol = tol_scale * sqrt((double)mt.p);
-    if (!(offmax > tol)) return;  // uniform for the whole CTA
-    if (tid == 0) atomicAdd(&rot_count[mi], 1);
-
-    // ---- T G T^H diagonal by parallel cyclic complex Jacobi (16 disjoint pairs per rotation set) ----
-    const double tol_in = 1e-15;
-    for (int sweep = 0; sweep < inner_sweeps; ++sweep) {
-        int any = 0;
-        for (int step = 0; step < JP - 1; ++step) {
-            if (tid < JB) {
-                int a, b;
-                if (tid == 0) {
-                    a = JP - 1;
-                    b = step;
-                } else {
-                    a = (step + tid) % (JP - 1);
-                    b = (step - tid + (JP - 1)) % (JP - 1);
-                }
-                const int p = a < b ? a : b, q = a < b ? b : a;
-                const double gpp = sGr[p * JLDG + p], gqq = sGr[q * JLDG + q];
-                const double gr = sGr[p * JLDG + q], gi = sGi[p * JLDG + q];
-                const double ag = hypot(gr, gi);
-                double c = 1.0, s = 0.0, er = 1.0, ei = 0.0;
-                if (gpp > defl2 && gqq > defl2 && ag > tol_in * sqrt(gpp) * sqrt(gqq)) {
-                    er = gr / ag;
-                    ei = gi / ag;
-                    const double aa = gqq - gpp, bb = 2.0 * ag;
-                    const double hh = hypot(aa, bb);
-                    const double tt = (aa >= 0.0) ? bb / (aa + hh) : bb / (aa - hh);
-                    c = rsqrt(1.0 + tt * tt);
-                    s = tt * c;
-                    any = 1;
-                }
-                pr_p[tid] = p;
-                pr_q[tid] = q;
-                cs_c[tid] = c;
-                cs_s[tid] = s;
-                cs_er[tid] = er;
-                cs_ei[tid] = ei;
-            }
-            __syncthreads();
-            // rows of G and T:  row p <- c x_p - s e x_q,  row q <- s x_p + c e x_q
-            for (int idx = tid; idx < 2 * JB * JP; idx += JTHREADS) {
-                const int which = idx / (JB * JP), jj = (idx / JP) % JB, col = idx % JP;
-                double *Xr = which ? sTr : sGr, *Xi = which ? sTi : sGi;
-                const int p = pr_p[jj], q = pr_q[jj];
-                const double c = cs_c[jj], s = cs_s[jj], er = cs_er[jj], ei = cs_ei[jj];
-                const double xpr = Xr[p * JLDG + col], xpi = Xi[p * JLDG + col];
-                const double xqr = Xr[q * JLDG + col], xqi = Xi[q * JLDG + col];
-                const double yr = er * xqr - ei * xqi, yi = er * xqi + ei * xqr;
-                Xr[p * JLDG + col] = c * xpr - s * yr;
-                Xi[p * JLDG + col] = c * xpi - s * yi;
-                Xr[q * JLDG + col] = s * xpr + c * yr;
-                Xi[q * JLDG + col] = s * xpi + c * yi;
-            }
-            __syncthreads();
-            // columns of G (G <- G T^H):  col p <- c y_p - s conj(e) y_q,  col q <- s y_p + c conj(e) y_q
-            for (int idx = tid; idx < JB * JP; idx += JTHREADS) {
-                const int jj = idx / JP, row = idx % JP;
-                const int p = pr_p[jj], q = pr_q[jj];
-                const double c = cs_c[jj], s = cs_s[jj], er = cs_er[jj], ei = cs_ei[jj];
-                const double ypr = sGr[row * JLDG + p], ypi = sGi[row * JLDG + p];
-                const double yqr = sGr[row * JLDG + q], yqi = sGi[row * JLDG + q];
-                const double zr = er * yqr + ei * yqi, zi = er * yqi - ei * yqr;
-                sGr[row * JLDG + p] = c * ypr - s * zr;
-                sGi[row * JLDG + p] = c * ypi - s * zi;
-                sGr[row * JLDG + q] = s * ypr + c * zr;
-                sGi[row * JLDG + q] = s * ypi + c * zi;
-            }
-            __syncthreads();
-        }
-        if (!__syncthreads_or(any)) break;
-    }
-    // rows of T ordered by descending eigenvalue (norm^2), ties by index.  The key is clamped at 0: the rotated diagonal of
-    // a row at rounding level can come out slightly negative and must not sort behind the all-zero padding rows (q..qp-1,
-    // always the last positions of a pair), or the padding content (zero Y, W = a unit vector outside the block) would
-    // move into a real row
-    if (tid < JP) {
-        const double di = fmax(sGr[tid * JLDG + tid], 0.0);
-        int rk = 0;
-        for (int k = 0; k < JP; ++k) {
-            const double dk = fmax(sGr[k * JLDG + k], 0.0);
-            if (dk > di || (dk == di && k < tid)) ++rk;
-        }
-        s_rank[tid] = rk;
-    }
-    __syncthreads();
-    double *QT = QTbuf + (int64_t)blockIdx.x * (2 * JP * JP);
-    for (int idx = tid; idx < JP * JP; idx += JTHREADS) {
-        const int i = idx / JP, k = idx % JP;
-        QT[s_rank[i] * JP + k] = sTr[i * JLDG + k];
-        QT[JP * JP + s_rank[i] * JP + k] = sTi[i * JLDG + k];
-    }
-    if (tid == 0) flags[blockIdx.x] = 1;
-}
-
-// grid (nsplit, pairs, 2): P <- T P (z = 0, rows of Y) and the same rows of W (z = 1)
-__global__ void __launch_bounds__(JTHREADS)
-    zjacobi_apply_kernel(double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ cta_mat,
-                         const int *__restrict__ rmap, int round, const double *__restrict__ QTbuf,
-                         const int *__restrict__ flags) {
-    extern __shared__ __align__(16) double jsmem[];
-    __shared__ int s_rows[JP];
-    const int pair = blockIdx.y;
-    if (!flags[pair]) return;
-    const JMat mt = mats[cta_mat[pair]];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, g = lane >> 2, t = lane & 3;
-    if (!j_pair_rows(mt, pair - mt.cta_begin, round, rmap, s_rows, tid)) return;
-    __syncthreads();
-    const double *QTr = QTbuf + (int64_t)pair * (2 * JP * JP), *QTi = QTr + JP * JP;
-    double qr[2][4][4], qi[2][4][4];
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-        for (int k8 = 0; k8 < 4; ++k8) {
-            const int o = (i * 16 + g) * JP + k8 * 8 + t;
-            qr[i][k8][0] = QTr[o];
-            qr[i][k8][1] = QTr[o + 8 * JP];
-            qr[i][k8][2] = QTr[o + 4];
-            qr[i][k8][3] = QTr[o + 8 * JP + 4];
-            qi[i][k8][0] = QTi[o];
-            qi[i][k8][1] = QTi[o + 8 * JP];
-            qi[i][k8][2] = QTi[o + 4];
-            qi[i][k8][3] = QTi[o + 8 * JP + 4];
-        }
-    double *Xr = work + (blockIdx.z ? mt.w_off : mt.y_off);
-    double *Xi = work + (blockIdx.z ? mt.wi_off : mt.yi_off);
-    const int ld = blockIdx.z ? mt.ldw : mt.ldy;
-    const int nch = (ld + JKC - 1) / JKC;
-    const int ch0 = blockIdx.x, chstep = gridDim.x;
-    if (ch0 >= nch) return;
-    j_load_chunk(jsmem, Xr, ld, s_rows, ch0 * JKC, tid);
-    j_load_chunk(jsmem + JP * JLDP, Xi, ld, s_rows, ch0 * JKC, tid);
-    cp_async_commit();
-    int it = 0;
-    for (int ch = ch0; ch < nch; ch += chstep, ++it) {
-        if (ch + chstep < nch) {
-            double *nxt = jsmem + ((it + 1) & 1) * ZJ_STAGE;
-            j_load_chunk(nxt, Xr, ld, s_rows, (ch + chstep) * JKC, tid);
-            j_load_chunk(nxt + JP * JLDP, Xi, ld, s_rows, (ch + chstep) * JKC, tid);
-        }
-        cp_async_commit();
-        cp_async_wait<1>();
-        __syncthreads();
-        const double *sr = jsmem + (it & 1) * ZJ_STAGE, *si = sr + JP * JLDP;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int nt = warp * 2 + h;
-            const int col = ch * JKC + nt * 8;
-            if (col < ld) {
-                double ar[2][4], ai[2][4];
-#pragma unroll
-                for (int i = 0; i < 2; ++i)
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) ar[i][e] = ai[i][e] = 0.0;
-#pragma unroll
-                for (int k8 = 0; k8 < 4; ++k8) {
-                    const int bo = (k8 * 8 + t) * JLDP + nt * 8 + g;
-                    double br[2] = {sr[bo], sr[bo + 4 * JLDP]}, bi[2] = {si[bo], si[bo + 4 * JLDP]};
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        double nqi[4] = {-qi[i][k8][0], -qi[i][k8][1], -qi[i][k8][2], -qi[i][k8][3]};
-                        dmma_16x8x8(ar[i], qr[i][k8], br);
-                        dmma_16x8x8(ar[i], nqi, bi);
-                        dmma_16x8x8(ai[i], qr[i][k8], bi);
-                        dmma_16x8x8(ai[i], qi[i][k8], br);
-                    }
-                }
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-#pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        const int64_t o = (int64_t)s_rows[i * 16 + g + 8 * hh] * ld + col + 2 * t;
-                        *reinterpret_cast<double2 *>(Xr + o) = make_double2(ar[i][2 * hh], ar[i][2 * hh + 1]);
-                        *reinterpret_cast<double2 *>(Xi + o) = make_double2(ai[i][2 * hh], ai[i][2 * hh + 1]);
-                    }
-                }
-            }
-        }
-        __syncthreads();
-    }
-    cp_async_wait<0>();
+    jacobi_apply_body<false>(jsmem, work, mats, cta_mat, rmap, round, QTbuf, flags, 0, 1, pair, 1);
 }
 
 // ---- init / finalize kernels ---------------------------------------------------------------------
@@ -1173,10 +960,7 @@ __global__ void __launch_bounds__(1024) jacobi_reorder_kernel(const double *__re
     __syncthreads();
     if (tid == 0) {
         const int n_act = s_nact;
-        int nb_act = (n_act + JB - 1) / JB;
-        if (nb_act < 2) nb_act = 2;
-        if (nb_act & 1) ++nb_act;
-        if (nb_act > mt.nb) nb_act = mt.nb;
+        const int nb_act = j_nb_act(n_act, mt.nb);
         mt.nb_act = nb_act;
         mt.n_act = n_act;
         act_out[2 * mi] = nb_act;
@@ -1355,7 +1139,7 @@ static void make_layout(int64_t nblocks, const int64_t *m, const int64_t *n, boo
 // directions -- they are moved (logically, through the row map) behind the active rows and never touched
 // again, so a numerically rank-deficient block only iterates on its significant rows.  Active rows are kept
 // ordered by descending norm (de Rijk).
-// cplx: the matrices are complex (layout made with cplx = true); the rounds run the zjacobi_* kernels
+// cplx: the matrices are complex (layout made with cplx = true); the rounds run the complex instantiations of the kernels
 static int run_jacobi(JLayout &L, char *work, cudaStream_t st, int32_t *info, int max_sweeps, bool cplx = false) {
     const int nmat = (int)L.mats.size();
     double *wf = reinterpret_cast<double *>(work);
@@ -1369,19 +1153,14 @@ static int run_jacobi(JLayout &L, char *work, cudaStream_t st, int32_t *info, in
     int *d_flags = reinterpret_cast<int *>(work + L.off_flags);
     static bool attr_set = false;
     if (!attr_set) {
-        B200_CUDA_CHECK(cudaFuncSetAttribute(jacobi_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             jacobi_smem_bytes()));
-        B200_CUDA_CHECK(cudaFuncSetAttribute(jacobi_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             jacobi_smem_bytes()));
-        B200_CUDA_CHECK(cudaFuncSetAttribute(jacobi_round_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             jacobi_smem_bytes()));
+        for (const void *k : {(const void *)jacobi_gram_kernel<false>, (const void *)jacobi_apply_kernel<false>,
+                              (const void *)jacobi_round_fused_kernel})
+            B200_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, jacobi_smem_bytes<false>()));
+        for (const void *k : {(const void *)jacobi_gram_kernel<true>, (const void *)jacobi_apply_kernel<true>})
+            B200_CUDA_CHECK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, jacobi_smem_bytes<true>()));
         // (q = 4096: 48 KB of keys and indices + the kernel's static shared memory is above the default limit)
         B200_CUDA_CHECK(cudaFuncSetAttribute(jacobi_reorder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              J_REORDER_MAX * 12));
-        B200_CUDA_CHECK(cudaFuncSetAttribute(zjacobi_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             zjacobi_smem_bytes()));
-        B200_CUDA_CHECK(cudaFuncSetAttribute(zjacobi_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             zjacobi_smem_bytes()));
         attr_set = true;
     }
     std::vector<int> rot((size_t)nmat), done((size_t)nmat, 0);
@@ -1405,6 +1184,25 @@ static int run_jacobi(JLayout &L, char *work, cudaStream_t st, int32_t *info, in
     std::vector<int> act((size_t)2 * nmat, 0);
     std::vector<double> nrm;
     std::vector<int> order;
+    // one round in three launches, the streaming phases over nsplit column splits: Gram partials, pivot solver, P <- Q^T P
+    // for Y and W.  Complex blocks always take it, with pivot solver 1
+    auto split_round = [&](auto cplx_tag, int nsplit) -> int {
+        constexpr bool CPLX = decltype(cplx_tag)::value;
+        jacobi_gram_kernel<CPLX><<<dim3((unsigned)nsplit, (unsigned)n_cta), JTHREADS, jacobi_smem_bytes<CPLX>(), st>>>(
+            wf, d_mats, d_cta, d_rmap, round_counter, d_done, d_G);
+        B200_CHECK_LAUNCH();
+        if (!CPLX && g_eig_variant == 3)
+            jacobi_eig_kernel_v3<<<n_cta, JTHREADS, 0, st>>>(d_mats, d_cta, d_rot, d_done, tol_scale, d_G, nsplit, d_QT,
+                                                           d_flags, g_eig_inner_sweeps, round_counter);
+        else
+            jacobi_eig_kernel<CPLX><<<n_cta, JTHREADS, 0, st>>>(d_mats, d_cta, d_rot, d_done, tol_scale, d_G, nsplit, d_QT,
+                                                                d_flags, CPLX ? std::max(1, g_eig_inner_sweeps) : J_INNER_SWEEPS);
+        B200_CHECK_LAUNCH();
+        jacobi_apply_kernel<CPLX><<<dim3((unsigned)nsplit, (unsigned)n_cta, 2), JTHREADS, jacobi_smem_bytes<CPLX>(), st>>>(
+            wf, d_mats, d_cta, d_rmap, round_counter, d_QT, d_flags);
+        B200_CHECK_LAUNCH();
+        return B200_OK;
+    };
     for (int sweep = 0; sweep < max_sweeps && ndone < nmat; ++sweep) {
         int rounds = 1;
         for (int i = 0; i < nmat; ++i)
@@ -1422,39 +1220,14 @@ static int run_jacobi(JLayout &L, char *work, cudaStream_t st, int32_t *info, in
         // small-block regime: all phases of a round in one launch (one CTA per pair, no column split)
         const bool fused = !cplx && g_eig_variant == 3 && max_ld <= g_fused_max_ld;
         for (int r = 0; r < rounds; ++r) {
-            if (cplx) {   // complex: always the three-launch round with column splits
-                zjacobi_gram_kernel<<<dim3((unsigned)nsplit, (unsigned)n_cta), JTHREADS, zjacobi_smem_bytes(), st>>>(
-                    wf, d_mats, d_cta, d_rmap, round_counter, d_done, d_G);
-                B200_CHECK_LAUNCH();
-                zjacobi_eig_kernel<<<n_cta, JTHREADS, 0, st>>>(d_mats, d_cta, d_rot, d_done, tol_scale, d_G, nsplit, d_QT,
-                                                               d_flags, std::max(1, g_eig_inner_sweeps));
-                B200_CHECK_LAUNCH();
-                zjacobi_apply_kernel<<<dim3((unsigned)nsplit, (unsigned)n_cta, 2), JTHREADS, zjacobi_smem_bytes(), st>>>(
-                    wf, d_mats, d_cta, d_rmap, round_counter, d_QT, d_flags);
-                B200_CHECK_LAUNCH();
-                ++round_counter;
-                continue;
-            }
             if (fused) {
-                jacobi_round_fused_kernel<<<n_cta, JTHREADS, jacobi_smem_bytes(), st>>>(
+                jacobi_round_fused_kernel<<<n_cta, JTHREADS, jacobi_smem_bytes<false>(), st>>>(
                     wf, d_mats, d_cta, d_rmap, round_counter, d_done, d_rot, tol_scale, d_G, d_QT, d_flags, g_eig_inner_sweeps);
                 B200_CHECK_LAUNCH();
-                ++round_counter;
-                continue;
+            } else {
+                const int rc = cplx ? split_round(std::true_type(), nsplit) : split_round(std::false_type(), nsplit);
+                if (rc) return rc;
             }
-            jacobi_gram_kernel<<<dim3((unsigned)nsplit, (unsigned)n_cta), JTHREADS, jacobi_smem_bytes(), st>>>(
-                wf, d_mats, d_cta, d_rmap, round_counter, d_done, d_G);
-            B200_CHECK_LAUNCH();
-            if (g_eig_variant == 3)
-                jacobi_eig_kernel_v3<<<n_cta, JTHREADS, 0, st>>>(d_mats, d_cta, d_rot, d_done, tol_scale, d_G, nsplit,
-                                                               d_QT, d_flags, g_eig_inner_sweeps, round_counter);
-            else
-                jacobi_eig_kernel<<<n_cta, JTHREADS, 0, st>>>(d_mats, d_cta, d_rot, d_done, tol_scale, d_G, nsplit, d_QT,
-                                                            d_flags);
-            B200_CHECK_LAUNCH();
-            jacobi_apply_kernel<<<dim3((unsigned)nsplit, (unsigned)n_cta, 2), JTHREADS, jacobi_smem_bytes(), st>>>(
-                wf, d_mats, d_cta, d_rmap, round_counter, d_QT, d_flags);
-            B200_CHECK_LAUNCH();
             ++round_counter;
         }
         jacobi_norms_kernel<<<dim3((unsigned)std::max(1, L.max_q), (unsigned)nmat), 128, 0, st>>>(wf, d_mats);
@@ -1498,10 +1271,7 @@ static int run_jacobi(JLayout &L, char *work, cudaStream_t st, int32_t *info, in
             std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return nrm[a] > nrm[b]; });
             int n_act = 0;
             while (n_act < mt.q && nrm[order[n_act]] > mt.defl) ++n_act;
-            int nb_act = (n_act + JB - 1) / JB;
-            if (nb_act < 2) nb_act = 2;
-            if (nb_act & 1) ++nb_act;
-            if (nb_act > mt.nb) nb_act = mt.nb;
+            const int nb_act = j_nb_act(n_act, mt.nb);
             int *rm = rmap.data() + mt.rmap_off;
             // physical padding rows (>= q) stay at the very end of the logical order
             for (int k = 0; k < mt.q; ++k) rm[k] = order[k];
@@ -1687,12 +1457,8 @@ static int block_svd_impl(int64_t nblocks, const int64_t *m, const int64_t *n, c
             if (mt.defl > 0.0) {
                 int n_act = 0;
                 while (n_act < mt.q && vn[pp[n_act]] > mt.defl * mt.defl) ++n_act;
-                int nb_act = (n_act + JB - 1) / JB;
-                if (nb_act < 2) nb_act = 2;
-                if (nb_act & 1) ++nb_act;
-                if (nb_act > mt.nb) nb_act = mt.nb;
                 mt.n_act = n_act;
-                mt.nb_act = nb_act;
+                mt.nb_act = j_nb_act(n_act, mt.nb);
                 changed = true;
             }
         }
