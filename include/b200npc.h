@@ -196,8 +196,8 @@ int b200_block_qr_f64(int64_t nblocks, const int64_t *m_host, const int64_t *n_h
 /* OUT[o, n, i] = sum_k M[n, k] T[o, k, i]  (T: outer x K x inner, OUT: outer x N x inner, row-major, i contiguous;
  * M: N x K on the device, K <= 32): a small matrix applied to the middle index without changing the layout.  Fuses the
  * two block transpositions and the skinny GEMM npc.tensordot needs for "W0.W1 applied to LP.theta" in the split-order
- * matvec (TwoSiteH.matvec, reference mps_common.py:1341-1343) into one streaming pass (default for dense tensors,
- * TwoSiteH.mpo_apply). */
+ * matvec (TwoSiteH.matvec, reference mps_common.py:1341-1343) into one streaming pass (taken for dense tensors with
+ * K <= 32, SplitOrderMatvec._apply_W01_fused). */
 int b200_mid_contract_f64(int64_t K, int64_t N, int64_t outer, int64_t inner, const double *M_dev, const double *T,
                           double *OUT, b200_stream_t stream);
 /* two-segment version: [OUT1; OUT2][o, n, i] = sum_k M[n, k] [T1; T2][o, k, i] with K = K1 + K2 rows taken from T1 then

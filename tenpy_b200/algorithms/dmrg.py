@@ -389,8 +389,6 @@ class TwoSiteDMRGEngine:
         """Reference mps_common.py:498."""
         self.eff_H = self.EffectiveH(self.env, self.i0, self.combine, self.move_right,
                                       matvec_order=self.options.get('matvec_order', 'auto'))
-        if 'mpo_apply' in self.options:
-            self.eff_H.mpo_apply = self.options['mpo_apply']
         if 'identity_env' in self.options:
             self.eff_H.identity_env = bool(self.options['identity_env'])
         # this engine's Lanczos calls `eff_H.deferred_check()` after its first read-back (and `diag` restarts on rejection)

@@ -166,33 +166,30 @@ def _get_RHeff(env, i, eff_H):
 
 
 class IdentityEnvRejected(Exception):
-    """raised by `TwoSiteH.deferred_check` when the environments turn out not to have identity components: the caller
-    restarts its iteration, the effective Hamiltonian has switched the shortcut off"""
+    """raised by `SplitOrderMatvec.deferred_check` when the environments turn out not to have identity components: the
+    caller restarts its iteration, the effective Hamiltonian has switched the shortcut off"""
 
 
-class TwoSiteH:
-    r"""Effective Hamiltonian ``LP--W0--W1--RP`` acting on the two-site wave function (reference :1245).
+class SplitOrderMatvec:
+    r"""The split-order routes of the two-site matvec, shared by the engine's `TwoSiteH` and the drop-in effective
+    Hamiltonian of the reference's engine (:func:`tenpy_b200.dropin.fast_two_site_engine`).  The class using it provides
+    ``i0, LP, RP, W0, W1, combine, pipeL, pipeR`` (as the reference's ``TwoSiteH`` with ``combine=True``) and ``_H_mpo``
+    (the MPO), and sends `matvec` to :meth:`_matvec_split` where :meth:`_use_split` says so.
 
-    With ``combine=True`` (default of the DMRG engine) `LHeff` (labels ``'(vR*.p0)', 'wR', '(vR.p0*)'``)
-    and `RHeff` (labels ``'wL', '(p1*.vL)', '(p1.vL*)'``) are formed once per bond and one `matvec` is two
-    contractions: ``LHeff . theta`` and ``(..) . RHeff``, dense cost :math:`4 D d^3 \chi^3` flops.
+    `matvec_order` (extension; same result, fewer flops): ``'combined'`` is the reference's sequence
+    ``LHeff . theta . RHeff``, dense cost :math:`4 D d^3 \chi^3` flops.  ``'split'`` keeps the combined interface (theta
+    with the pipes ``(vL.p0)``, ``(p1.vR)``; `LHeff`/`RHeff` are still formed for the environment update and the mixer)
+    but applies ``LP``, the two-site MPO tensor ``W0.W1`` and ``RP`` one after the other to the split theta -- the
+    contraction order of the reference's ``combine=False`` branch (:1340), dense cost :math:`4 D d^2 \chi^3 + O(\chi^2)`,
+    i.e. `d` times fewer flops in the two large GEMMs.  ``'auto'`` (default) takes ``'split'`` when the largest block of
+    theta has at least ``SPLIT_MIN_BLOCK`` elements (compute-bound regime) and ``'combined'`` for small ragged blocks,
+    where the number of launches decides.
 
-    `matvec_order` (extension; same result, fewer flops): ``'combined'`` is the reference's sequence above.
-    ``'split'`` keeps the combined interface (theta with the pipes ``(vL.p0)``, ``(p1.vR)``; `LHeff`/`RHeff`
-    are still formed for the environment update and the mixer) but applies ``LP``, the two-site MPO tensor
-    ``W0.W1`` and ``RP`` one after the other to the split theta -- the contraction order of the reference's
-    ``combine=False`` branch (:1340), dense cost :math:`4 D d^2 \chi^3 + O(\chi^2)`, i.e. `d` times fewer
-    flops in the two large GEMMs at the price of two block transpositions of the ``D d^2 \chi^2``
-    intermediate.  ``'auto'`` (default) takes ``'split'`` when the largest block of theta has at least
-    ``SPLIT_MIN_BLOCK`` elements (compute-bound regime) and ``'combined'`` for small ragged blocks, where
-    the number of launches decides."""
-    length = 2
-    acts_on = ['vL', 'p0', 'p1', 'vR']
+    The shapes alone choose how ``W0.W1`` is applied: to dense tensors (one block) with ``K = D d^2 <= 32`` contracted
+    rows (``K1 + K2 = (D-1) d^2 + d^2`` without the identity components) by the streaming kernel b200_mid_contract(2)_f64,
+    which keeps the layout; otherwise by `npc.tensordot` (two block transpositions and a skinny GEMM)."""
     SPLIT_MIN_BLOCK = 1 << 20
-    # 'fused' (default): W0.W1 is applied to LP.theta by the streaming kernel b200_mid_contract(2)_f64 where it applies
-    # (no charges / one block);
-    # 'tensordot': always by npc.tensordot (two block transpositions + a skinny GEMM).
-    mpo_apply = 'fused'
+    matvec_order = 'auto'
     # skip the identity components of the environments in the split-order matvec (see _identity_env_setup): host logic on
     # the GPU-verified kernels, results checked against the reference goldens; engine option `identity_env` switches it off
     identity_env = True
@@ -203,31 +200,14 @@ class TwoSiteH:
     identity_check = 'immediate'
     stats = {'identity_env_bonds': 0, 'identity_env_rejected': 0}     # diagnostics (how often the shortcut applied)
 
-    def __init__(self, env, i0, combine=False, move_right=True, matvec_order='auto'):
-        if matvec_order not in ('auto', 'combined', 'split'):
-            raise ValueError('matvec_order has to be one of auto, combined, split')
-        self.matvec_order = matvec_order
-        self._W01 = None
-        self.i0 = i0
-        self.LP = env.get_LP(i0)
-        self.RP = env.get_RP(i0 + 1)
-        self.W0 = env.H.get_W(i0).replace_labels(['p', 'p*'], ['p0', 'p0*'])
-        self.W1 = env.H.get_W(i0 + 1).replace_labels(['p', 'p*'], ['p1', 'p1*'])
-        self.dtype = env.H.dtype
-        self._H_mpo = env.H
-        self.combine = combine
-        self.N = (self.LP.get_leg('vR').ind_len * self.W0.get_leg('p0').ind_len *
-                  self.W1.get_leg('p1').ind_len * self.RP.get_leg('vL').ind_len)
-        if combine:
-            self.combine_Heff(env)
-
-    def matvec(self, theta):
-        """Apply the effective Hamiltonian to `theta` (reference mps_common.py:1321)."""
-        labels = theta.get_leg_labels()
-        if self.combine and self._use_split(theta):
-            return self._matvec_split(theta, labels)
-        chain, relabel = _TWO_SITE_CHAINS['combined' if self.combine else 'plain']
-        return _apply_chain(self, theta, chain, relabel).itranspose(labels)
+    # per-instance state, made by the routes on first use
+    _W01 = _W01_mat = _RP_t = None                     # W0.W1; plain split order: W0.W1 as a matrix, RP transposed
+    _id_env = None                                     # identity shortcut: None until decided, then True / False
+    _id_check = None                                   # its pending deferred test
+    _LP_rest = _RP_rest = _leg_IdL = _leg_IdR = _W01p = _mask_rest_r = _mpo_cache = None   # see _identity_env_prepare
+    _M_id = _N1 = _fused_legs = _RP_rest_t = None      # fused identity route, see _bind_fused_identity
+    _dense_recipe = None                               # replayed kernel sequence, see _dense_recipe_bind
+    _dense_recipe_off = False
 
     def _use_split(self, theta):
         if self.matvec_order == 'auto':
@@ -235,17 +215,22 @@ class TwoSiteH:
             return len(sizes) > 0 and int(sizes.max()) >= self.SPLIT_MIN_BLOCK
         return self.matvec_order == 'split'
 
+    def _combine_result(self, out, labels):
+        """``out[vL, p0, p1, vR]`` (ours) with the pipes and the label order of theta"""
+        out = out.combine_legs([['vL', 'p0'], ['p1', 'vR']], pipes=[self.pipeL, self.pipeR], _view=True)
+        return out.itranspose(labels)
+
     def _matvec_split(self, theta, labels):
         """``LP . theta . (W0 W1) . RP`` on the split legs; interface (labels, pipes) of the combined matvec."""
         if self._W01 is None:
             self._W01 = npc.tensordot(self.W0, self.W1, axes=['wR', 'wL'])   # wL p0 p0* p1 p1* wR  (D^2 d^4 numbers)
-        rec = getattr(self, '_dense_recipe', None)
-        if rec is None and not self._dense_recipe_off and self.identity_env and self.mpo_apply == 'fused':
+        rec = self._dense_recipe
+        if rec is None and not self._dense_recipe_off and self.identity_env:
             rec = self._dense_recipe_from_cache(theta)
-        if rec is not None and theta._layout is rec['lay'] and theta._labels == rec['labels']:
+        if rec is not None and theta._layout is rec['theta_lay'] and theta._labels == rec['labels']:
             return self._dense_recipe_run(theta, rec)
         th = theta.split_legs(['(vL.p0)', '(p1.vR)'], _view=True)            # vL p0 p1 vR (read only here)
-        if self.identity_env and getattr(self, '_id_env', None) is not False:
+        if self.identity_env and self._id_env is not False:
             try:
                 if self._identity_env_setup():
                     return self._matvec_split_identity(th, labels)
@@ -254,15 +239,13 @@ class TwoSiteH:
                 logging.getLogger(__name__).warning('identity_env shortcut disabled for bond %d: %r', self.i0, e)
                 self._id_env = False
         th = _mv_dot(self.LP, th, axes=['vR', 'vL'])                          # vR* wR p0 p1 vR      2 D d^2 chi^3
-        fused = self._apply_W01_fused(th) if self.mpo_apply == 'fused' else None
+        fused = self._apply_W01_fused(th)
         if fused is not None:
             th = _mv_dot(fused, self._RP_t, axes=[['wR', 'vR'], ['wL', 'vL']])          # no transposition left
         else:
             th = npc.tensordot(th, self._W01, axes=[['wR', 'p0', 'p1'], ['wL', 'p0*', 'p1*']])  # vR* vR p0 p1 wR
             th = _mv_dot(th, self.RP, axes=[['vR', 'wR'], ['vL', 'wL']])          # vR* p0 p1 vL*   2 D d^2 chi^3
-        th.ireplace_labels(['vR*', 'vL*'], ['vL', 'vR'])
-        th = th.combine_legs([['vL', 'p0'], ['p1', 'vR']], pipes=[self.pipeL, self.pipeR], _view=True)  # th is ours
-        return th.itranspose(labels)
+        return self._combine_result(th.ireplace_labels(['vR*', 'vL*'], ['vL', 'vR']), labels)   # th is ours
 
     def _identity_env_setup(self):
         """In mixed canonical form the component ``wR = IdL`` of `LP` and ``wL = IdR`` of `RP` are identity matrices
@@ -270,18 +253,18 @@ class TwoSiteH:
         per bond (``|LP[IdL] - 1| <= 1e-11 sqrt(chi)``, same for `RP`); if it holds, the matvec skips these components:
         ``D - 1`` instead of ``D`` large GEMMs on either side.  Prepares `LP` / `RP` without, and ``W0.W1`` with the
         identity components moved to the end of its MPO legs.  Returns False (and remembers it) if not applicable."""
-        if getattr(self, '_id_env', None) is not None:
+        if self._id_env is not None:
             return self._id_env
         self._id_env = False
         ok = self._identity_env_prepare()
-        TwoSiteH.stats['identity_env_bonds' if ok else 'identity_env_rejected'] += 1
+        SplitOrderMatvec.stats['identity_env_bonds' if ok else 'identity_env_rejected'] += 1
         self._id_env = ok
         return ok
 
     def deferred_check(self):
         """Called by the eigensolver right after one of its own device synchronisations: evaluates the pending test of the
         identity-environment shortcut (free now); raises `IdentityEnvRejected` if it failed."""
-        pending = getattr(self, '_id_check', None)
+        pending = self._id_check
         if not pending:
             return
         self._id_check = None
@@ -291,14 +274,12 @@ class TwoSiteH:
                 self._id_env = False
                 self._dense_recipe = None
                 self._dense_recipe_off = True
-                TwoSiteH.stats['identity_env_bonds'] -= 1
-                TwoSiteH.stats['identity_env_rejected'] += 1
+                SplitOrderMatvec.stats['identity_env_bonds'] -= 1
+                SplitOrderMatvec.stats['identity_env_rejected'] += 1
                 raise IdentityEnvRejected('environment component differs from the identity')
 
     def _identity_env_prepare(self):
-        H = getattr(self, '_H_mpo', None)
-        if H is None:
-            return False
+        H = self._H_mpo
         IdL, IdR = H.get_IdL(self.i0), H.get_IdR(self.i0 + 1)
         if IdL is None or IdR is None or getattr(H, 'explicit_plus_hc', False):
             return False
@@ -348,8 +329,6 @@ class TwoSiteH:
         cache = H.__dict__.setdefault('_b200_two_site_cache', {})
         ent = cache.get(self.i0)
         if ent is None:
-            if self._W01 is None:
-                self._W01 = npc.tensordot(self.W0, self.W1, axes=['wR', 'wL'])
             W_rest, W_one = pieces(self._W01, 'wL', only_l)
             W01p = npc.concatenate([W_rest, W_one], axis='wL')                   # wL: [others ..., IdL]
             W_rest, W_one = pieces(W01p, 'wR', only_r)
@@ -362,41 +341,18 @@ class TwoSiteH:
     def _matvec_split_identity(self, th, labels):
         """Split-order matvec without the identity components of the environments: ``T1 = [LP_rest . theta, theta]``,
         ``T2 = (W0 W1) . T1``, ``result = T2[rest] . RP_rest + T2[IdR]``."""
-        cat = getattr(self, '_t1_cat', None)
-        if cat is not None and self.mpo_apply != 'fused' and th._layout is cat[3]:
-            # no charges: GEMM 1 writes straight into the first block of the packed [LP_rest . theta, theta], theta is
-            # copied behind it (no add_leg / concatenate launches)
-            lay_cat, legs_cat, n0, _ = cat
-            from .. import backend
-            buf = backend.empty(lay_cat.size)
-            _mv_dot(self._LP_rest, th, axes=['vR', 'vL'], _out=buf[:n0])
-            buf[n0:].copy_(th._buf[:lay_cat.size - n0])
-            t1 = npc.Array(legs_cat, np.float64, th.qtotal, ['vR*', 'wR', 'p0', 'p1', 'vR'])._set_blocks(lay_cat, buf)
-            return self._matvec_split_identity_tail(t1, labels)
         t1 = _mv_dot(self._LP_rest, th, axes=['vR', 'vL'])                    # vR* wR' p0 p1 vR   2 (D-1) d^2 chi^3
-        if self.mpo_apply == 'fused':
-            fused = self._apply_W01_fused_identity(t1, th)
-            if fused is not None:
-                y_rest, y_id = fused                                         # vR* p0 p1 wR' vR ; vR* p0 p1 vR
-                out = _mv_dot(y_rest, self._RP_rest_t, axes=[['wR', 'vR'], ['wL', 'vL']])
-                out.ireplace_labels(['vR*', 'vL*'], ['vL', 'vR'])
-                out.iadd_prefactor_other(1., y_id.ireplace_label('vR*', 'vL'))
-                out = out.combine_legs([['vL', 'p0'], ['p1', 'vR']], pipes=[self.pipeL, self.pipeR], _view=True)
-                out = out.itranspose(labels)
-                self._dense_recipe_record(th, t1, y_rest, y_id, out)
-                return out
-        n0_single = int(t1._layout.size) if (t1._layout.nblocks == 1 and not t1._layout.has_padding) else None
+        fused = self._apply_W01_fused_identity(t1, th)
+        if fused is not None:
+            y_rest, y_id = fused                                             # vR* p0 p1 wR' vR ; vR* p0 p1 vR
+            out = _mv_dot(y_rest, self._RP_rest_t, axes=[['wR', 'vR'], ['wL', 'vL']])
+            out.ireplace_labels(['vR*', 'vL*'], ['vL', 'vR'])
+            out.iadd_prefactor_other(1., y_id.ireplace_label('vR*', 'vL'))
+            out = self._combine_result(out, labels)
+            self._dense_recipe_record(th, t1, y_rest, y_id, out)
+            return out
         th_id = th.add_leg(self._leg_IdL, 0, axis=1, label='wR').ireplace_label('vL', 'vR*')
         t1 = npc.concatenate([t1, th_id], axis='wR')                         # wR: [others ..., IdL]
-        lay = t1._layout
-        if n0_single is not None and th._layout.nblocks == 1 and not th._layout.has_padding and lay.nblocks == 2 and \
-                not lay.has_padding and list(lay.offsets) == [0, n0_single] and int(lay.sizes[1]) == int(th._layout.size) \
-                and t1.get_leg_labels() == ['vR*', 'wR', 'p0', 'p1', 'vR']:
-            self._t1_cat = (lay, list(t1.legs), n0_single, th._layout)      # structure for the direct-write path
-        return self._matvec_split_identity_tail(t1, labels)
-
-    def _matvec_split_identity_tail(self, t1, labels):
-        """second half of :meth:`_matvec_split_identity`: ``(W0 W1) . T1``, contraction with `RP_rest`, identity part"""
         t2 = npc.tensordot(t1, self._W01p, axes=[['wR', 'p0', 'p1'], ['wL', 'p0*', 'p1*']])   # vR* vR p0 p1 wR
         views = self._split_t2_views(t2)
         if views is not None:            # no charges: the two components are the two blocks of t2, shared not copied
@@ -408,17 +364,19 @@ class TwoSiteH:
         out.ireplace_labels(['vR*', 'vL*'], ['vL', 'vR'])
         direct.ireplace_label('vR*', 'vL').itranspose(out.get_leg_labels())
         out.iadd_prefactor_other(1., direct)
-        out = out.combine_legs([['vL', 'p0'], ['p1', 'vR']], pipes=[self.pipeL, self.pipeR], _view=True)
-        return out.itranspose(labels)
+        return self._combine_result(out, labels)
 
     # The dense (no charges, one block per tensor) identity-environment matvec is always the same six kernels: split theta,
     # int8 GEMM with LP_rest, W0 W1 streaming pass, split, int8 GEMM with RP_rest, axpy.  Going through the Array layer
     # (label bookkeeping, leg checks, plan look-ups, result objects) costs ~1 ms of Python per matvec -- as much as the
-    # kernels take at chi = 1024 -- so after the first call of a bond the raw sequence is replayed on the buffers.
+    # kernels take at chi = 1024 -- so after the first call of a bond the raw sequence is replayed on the buffers.  The
+    # geometry of the sequence depends on the MPO and the shapes only: it is kept in the per-bond cache on the MPO, so that
+    # later visits of the bond replay it from their first matvec on.
     def _dense_recipe_record(self, th, t1, y_rest, y_id, out):
-        if getattr(self, '_dense_recipe', None) is not None or self._dense_recipe_off:
+        """first call of a bond on the fused identity route: record the geometry of its kernels and bind it (`out` is the
+        template of the results)"""
+        if self._dense_recipe is not None or self._dense_recipe_off:
             return
-        from .. import backend
         arrs = (th, t1, y_rest, y_id, out, self._LP_rest, self._RP_rest_t)
         if any(a._layout.nblocks != 1 for a in arrs) or np.any(out.qtotal != th.qtotal):
             self._dense_recipe_off = True
@@ -433,53 +391,44 @@ class TwoSiteH:
         if plan1 is None or plan2 is None:
             self._dense_recipe_off = True
             return
-        ent = getattr(self, '_mpo_cache', None)
-        if ent is not None:
-            ent['recipe_geom'] = {'theta_lay': out._layout, 'labels': list(out._labels), 'plan1': plan1[2], 'plan2': plan2[2],
-                                  'shape_t1': tuple(t1.shape), 'n_t1': int(t1._layout.size), 'n_yr': int(y_rest._layout.size),
-                                  'n_yi': int(y_id._layout.size),
-                                  'padded': any(a._layout.has_padding for a in (t1, y_rest, y_id, out))}
-        self._dense_recipe = {
-            'lay': out._layout, 'labels': list(out._labels), 'template': out,
-            'g1': (chi_l * Dm1, d0 * d1 * chi_r, chi_l), 'plan1': plan1[2],          # (m, n, k) of LP_rest . theta
-            'g2': (chi_l * d0 * d1, chi_r, Dm1 * chi_r), 'plan2': plan2[2],          # y_rest . RP_rest
-            'mid': (Dm1 * d0 * d1, d0 * d1, self._N1, d0 * d1, chi_l, chi_r),
-            'n_t1': int(t1._layout.size), 'n_yr': int(y_rest._layout.size), 'n_yi': int(y_id._layout.size),
+        geom = self._mpo_cache['recipe_geom'] = {
+            'theta_lay': out._layout, 'labels': list(out._labels), 'plan1': plan1[2], 'plan2': plan2[2],
+            'shape_t1': tuple(t1.shape), 'n_t1': int(t1._layout.size), 'n_yr': int(y_rest._layout.size),
+            'n_yi': int(y_id._layout.size),
             # buffers whose size is not a multiple of the block alignment carry zero padding (BLAS-1 runs over it)
-            'alloc': backend.zeros if any(a._layout.has_padding for a in (t1, y_rest, y_id, out)) else backend.empty,
-        }
-
-    _dense_recipe_off = False
+            'padded': any(a._layout.has_padding for a in (t1, y_rest, y_id, out))}
+        self._dense_recipe_bind(geom, out)
 
     def _dense_recipe_from_cache(self, theta):
         """From the second visit of a bond on (same MPO, same shapes) the kernel sequence is known before the first matvec:
         set up the identity components and bind the recorded geometry to this bond's buffers -- the Array-level route is
         not taken at all.  None if the bond has no recorded geometry (first visit) or anything differs."""
-        H = getattr(self, '_H_mpo', None)
-        ent = None if H is None else H.__dict__.get('_b200_two_site_cache', {}).get(self.i0)
+        ent = self._H_mpo.__dict__.get('_b200_two_site_cache', {}).get(self.i0)
         geom = None if ent is None else ent.get('recipe_geom')
         if geom is None or 'M_id' not in ent or theta._layout is not geom['theta_lay'] or theta._labels != geom['labels']:
             return None
-        if getattr(self, '_id_env', None) is False or not self._identity_env_setup():
+        if self._id_env is False or not self._identity_env_setup():
             return None
         chi_l, Dm1, d0, d1, chi_r = geom['shape_t1']
         if self._LP_rest.shape != (chi_l, Dm1, chi_l) or self._RP_rest.get_leg('wL').ind_len != Dm1 or \
                 self._LP_rest._layout.nblocks != 1 or self._RP_rest._layout.nblocks != 1:
             return None
-        from .. import backend
-        self._M_id, self._N1, self._fused_legs = ent['M_id'], ent['N1'], ent['fused_legs']
-        self._RP_rest_t = self._RP_rest.transpose(['wL', 'vL', 'vL*'])
-        self._RP_rest_t._oz_const = True
+        self._bind_fused_identity(ent)
         if self._RP_rest_t.shape != (Dm1, chi_r, chi_r):
             return None
-        self._dense_recipe = {
-            'lay': geom['theta_lay'], 'labels': geom['labels'], 'template': theta.copy(deep=False),
-            'g1': (chi_l * Dm1, d0 * d1 * chi_r, chi_l), 'plan1': geom['plan1'],
-            'g2': (chi_l * d0 * d1, chi_r, Dm1 * chi_r), 'plan2': geom['plan2'],
-            'mid': (Dm1 * d0 * d1, d0 * d1, self._N1, d0 * d1, chi_l, chi_r),
-            'n_t1': geom['n_t1'], 'n_yr': geom['n_yr'], 'n_yi': geom['n_yi'],
-            'alloc': backend.zeros if geom['padded'] else backend.empty,
-        }
+        return self._dense_recipe_bind(geom, theta.copy(deep=False))
+
+    def _dense_recipe_bind(self, geom, template):
+        """the replayed kernel sequence of this bond: the recorded geometry, the launch shapes derived from it, and
+        `template`, an Array with the layout and labels of the results whose buffer each call replaces"""
+        from .. import backend
+        chi_l, Dm1, d0, d1, chi_r = geom['shape_t1']
+        self._dense_recipe = dict(
+            geom, template=template,
+            g1=(chi_l * Dm1, d0 * d1 * chi_r, chi_l),                      # (m, n, k) of LP_rest . theta
+            g2=(chi_l * d0 * d1, chi_r, Dm1 * chi_r),                      # y_rest . RP_rest
+            mid=(Dm1 * d0 * d1, d0 * d1, self._N1, d0 * d1, chi_l, chi_r),
+            alloc=backend.zeros if geom['padded'] else backend.empty)
         return self._dense_recipe
 
     def _dense_recipe_run(self, theta, rec):
@@ -492,9 +441,10 @@ class TwoSiteH:
         y_r, y_i = alloc(rec['n_yr']), alloc(rec['n_yi'])
         K1, K2, N1, N2, chi_l, chi_r = rec['mid']
         lib.mid_contract2(K1, K2, N1, N2, chi_l, chi_r, self._M_id, t1, theta._buf, y_r, y_i)
-        out = alloc(rec['lay'].size)
+        n = rec['theta_lay'].size
+        out = alloc(n)
         npc._raw_product(lib, y_r, self._RP_rest_t, rec['g2'], rec['plan2'], out, s)
-        lib.axpy(rec['lay'].size, 1., y_i, out)
+        lib.axpy(n, 1., y_i, out)
         res = rec['template'].copy(deep=False)
         res._buf = out
         return res
@@ -529,6 +479,12 @@ class TwoSiteH:
         direct._set_blocks(lay_d, t2._buf[o1:o1 + n1])
         return rest, direct
 
+    def _bind_fused_identity(self, ent):
+        """bind the per-bond constants of the fused identity route (`ent`: the bond's entry of the cache on the MPO)"""
+        self._M_id, self._N1, self._fused_legs = ent['M_id'], ent['N1'], ent['fused_legs']
+        self._RP_rest_t = self._RP_rest.transpose(['wL', 'vL', 'vL*'])
+        self._RP_rest_t._oz_const = True
+
     def _apply_W01_fused_identity(self, t1, th):
         """``[Y_rest; Y_IdR] = (W0 W1) . [T1_rest; theta]`` in one streaming pass (b200_mid_contract2_f64): both inputs
         are read once, both outputs come out in the layout their consumer wants.  Dense (one block) only; None if not
@@ -541,31 +497,25 @@ class TwoSiteH:
         K1, K2 = Dm1 * d0 * d1, d0 * d1
         if K1 + K2 > 32:
             return None
-        ent = getattr(self, '_mpo_cache', None)
-        if getattr(self, '_M_id', None) is None and ent is not None and 'M_id' in ent:
-            self._M_id, self._N1, self._fused_legs = ent['M_id'], ent['N1'], ent['fused_legs']
-            self._RP_rest_t = self._RP_rest.transpose(['wL', 'vL', 'vL*'])
-            self._RP_rest_t._oz_const = True
-        if getattr(self, '_M_id', None) is None:
-            # (W0 W1) as a matrix [(p0' p1' wR), (wL p0 p1)] with the identity components moved to the end of both
-            # index groups; D^2 d^4 model constants, permuted on the host once per bond (and kept on the MPO)
-            H = self._H_mpo
-            IdL, IdR = H.get_IdL(self.i0), H.get_IdR(self.i0 + 1)
-            W = self._W01.transpose(['p0', 'p1', 'wR', 'wL', 'p0*', 'p1*']).to_ndarray()
-            D_r, D_l = W.shape[2], W.shape[3]
-            rest_r = [x for x in range(D_r) if x != IdR]
-            rest_l = [x for x in range(D_l) if x != IdL]
-            rows = np.concatenate([W[:, :, rest_r].reshape(d0 * d1 * len(rest_r), D_l, d0, d1),
-                                   W[:, :, IdR].reshape(d0 * d1, D_l, d0, d1)], axis=0)
-            M = np.concatenate([rows[:, rest_l].reshape(rows.shape[0], -1), rows[:, IdL].reshape(rows.shape[0], -1)],
-                               axis=1)
-            self._M_id = backend.to_device(np.ascontiguousarray(M))
-            self._RP_rest_t = self._RP_rest.transpose(['wL', 'vL', 'vL*'])
-            self._RP_rest_t._oz_const = True
-            self._N1 = d0 * d1 * len(rest_r)
-            self._fused_legs = (self._W01.get_leg('p0'), self._W01.get_leg('p1'), self._RP_rest.get_leg('wL').conj())
-            if ent is not None:
-                ent.update({'M_id': self._M_id, 'N1': self._N1, 'fused_legs': self._fused_legs})
+        if self._M_id is None:
+            ent = self._mpo_cache
+            if 'M_id' not in ent:
+                # (W0 W1) as a matrix [(p0' p1' wR), (wL p0 p1)] with the identity components moved to the end of both
+                # index groups; D^2 d^4 model constants, permuted on the host once per bond (and kept on the MPO)
+                H = self._H_mpo
+                IdL, IdR = H.get_IdL(self.i0), H.get_IdR(self.i0 + 1)
+                W = self._W01.transpose(['p0', 'p1', 'wR', 'wL', 'p0*', 'p1*']).to_ndarray()
+                D_r, D_l = W.shape[2], W.shape[3]
+                rest_r = [x for x in range(D_r) if x != IdR]
+                rest_l = [x for x in range(D_l) if x != IdL]
+                rows = np.concatenate([W[:, :, rest_r].reshape(d0 * d1 * len(rest_r), D_l, d0, d1),
+                                       W[:, :, IdR].reshape(d0 * d1, D_l, d0, d1)], axis=0)
+                M = np.concatenate([rows[:, rest_l].reshape(rows.shape[0], -1), rows[:, IdL].reshape(rows.shape[0], -1)],
+                                   axis=1)
+                ent.update({'M_id': backend.to_device(np.ascontiguousarray(M)), 'N1': d0 * d1 * len(rest_r),
+                            'fused_legs': (self._W01.get_leg('p0'), self._W01.get_leg('p1'),
+                                           self._RP_rest.get_leg('wL').conj())})
+            self._bind_fused_identity(ent)
         N1, N2 = self._N1, K2
         p0leg, p1leg, wleg = self._fused_legs
         legs_r = [t1.legs[0], p0leg, p1leg, wleg, t1.legs[4]]
@@ -587,9 +537,8 @@ class TwoSiteH:
         W01 = self._W01
         if th._layout.nblocks != 1 or W01._layout.nblocks != 1 or th.get_leg_labels() != ['vR*', 'wR', 'p0', 'p1', 'vR']:
             return None
-        if getattr(self, '_W01_mat', None) is None:
-            M = W01.transpose(['p0', 'p1', 'wR', 'wL', 'p0*', 'p1*'])        # [(p0' p1' wR'), (wL p0 p1)], one block
-            self._W01_mat = M
+        if self._W01_mat is None:
+            self._W01_mat = W01.transpose(['p0', 'p1', 'wR', 'wL', 'p0*', 'p1*'])   # [(p0' p1' wR'), (wL p0 p1)], one block
             self._RP_t = self.RP.transpose(['wL', 'vL', 'vL*'])
         M = self._W01_mat
         chi_l, D, d0, d1, chi_r = th.shape
@@ -604,6 +553,42 @@ class TwoSiteH:
         buf = backend.zeros(lay.size) if lay.has_padding else backend.empty(lay.size)
         backend.get_lib().mid_contract(K, N, chi_l, chi_r, M._buf, th._buf, buf)
         return res._set_blocks(lay, buf)
+
+
+class TwoSiteH(SplitOrderMatvec):
+    r"""Effective Hamiltonian ``LP--W0--W1--RP`` acting on the two-site wave function (reference :1245).
+
+    With ``combine=True`` (default of the DMRG engine) `LHeff` (labels ``'(vR*.p0)', 'wR', '(vR.p0*)'``)
+    and `RHeff` (labels ``'wL', '(p1*.vL)', '(p1.vL*)'``) are formed once per bond and one `matvec` is two
+    contractions: ``LHeff . theta`` and ``(..) . RHeff``, dense cost :math:`4 D d^3 \chi^3` flops.  `matvec_order`
+    chooses between that order and the split order of :class:`SplitOrderMatvec`."""
+    length = 2
+    acts_on = ['vL', 'p0', 'p1', 'vR']
+
+    def __init__(self, env, i0, combine=False, move_right=True, matvec_order='auto'):
+        if matvec_order not in ('auto', 'combined', 'split'):
+            raise ValueError('matvec_order has to be one of auto, combined, split')
+        self.matvec_order = matvec_order
+        self.i0 = i0
+        self.LP = env.get_LP(i0)
+        self.RP = env.get_RP(i0 + 1)
+        self.W0 = env.H.get_W(i0).replace_labels(['p', 'p*'], ['p0', 'p0*'])
+        self.W1 = env.H.get_W(i0 + 1).replace_labels(['p', 'p*'], ['p1', 'p1*'])
+        self.dtype = env.H.dtype
+        self._H_mpo = env.H
+        self.combine = combine
+        self.N = (self.LP.get_leg('vR').ind_len * self.W0.get_leg('p0').ind_len *
+                  self.W1.get_leg('p1').ind_len * self.RP.get_leg('vL').ind_len)
+        if combine:
+            self.combine_Heff(env)
+
+    def matvec(self, theta):
+        """Apply the effective Hamiltonian to `theta` (reference mps_common.py:1321)."""
+        labels = theta.get_leg_labels()
+        if self.combine and self._use_split(theta):
+            return self._matvec_split(theta, labels)
+        chain, relabel = _TWO_SITE_CHAINS['combined' if self.combine else 'plain']
+        return _apply_chain(self, theta, chain, relabel).itranspose(labels)
 
     def combine_Heff(self, env, left=True, right=True):
         """Reference mps_common.py:1350.  The pipes are made from the legs right away; the contractions

@@ -23,7 +23,8 @@ reference asserts at ``tenpy/linalg/__init__.py:74`` that its ``@use_cython`` de
 The speed-relevant extension of the engine -- the split-order / identity-environment effective-H matvec -- plugs into the
 reference engine through the reference's own hook, the class attribute ``EffectiveH`` (tenpy/algorithms/mps_common.py:
 ``Sweep.EffectiveH``): :func:`fast_two_site_engine` returns a subclass of the reference's ``TwoSiteDMRGEngine`` whose
-``EffectiveH`` is the reference's ``TwoSiteH`` with ``matvec`` replaced by the device-optimised contraction order.
+``EffectiveH`` inherits the reference's ``TwoSiteH`` and the engine's split-order routes
+(:class:`tenpy_b200.algorithms.mps_common.SplitOrderMatvec`, the same code the engine's own ``TwoSiteH`` runs).
 """
 import importlib
 import importlib.abc
@@ -101,34 +102,21 @@ def fast_two_site_engine():
         raise RuntimeError('call tenpy_b200.dropin.install() first')
     from tenpy.algorithms import dmrg as ref_dmrg
     from tenpy.algorithms import mps_common as ref_common
-    from .algorithms.mps_common import TwoSiteH as _EngineH
+    from .algorithms.mps_common import SplitOrderMatvec
 
-    class B200TwoSiteH(ref_common.TwoSiteH):
+    class B200TwoSiteH(SplitOrderMatvec, ref_common.TwoSiteH):
         """reference ``TwoSiteH`` (same constructor, attributes, `combine_theta`, `update_LP` ...); `matvec` applies
         ``LP``, ``W0 W1``, ``RP`` to the split theta without the identity components of the environments where that is
-        cheaper (tenpy_b200.algorithms.mps_common.TwoSiteH._matvec_split), the reference order otherwise."""
+        cheaper (`SplitOrderMatvec`), the reference order otherwise."""
 
         def __init__(self, env, i0, combine=False, move_right=True):
             super().__init__(env, i0, combine, move_right)
             self._H_mpo = env.H
-            self._W01 = None
-            self._LHeff = getattr(self, 'LHeff', None)
-            self._RHeff = getattr(self, 'RHeff', None)
-
-        matvec_order = 'auto'
 
         def matvec(self, theta):
             if self.combine and self._use_split(theta):
                 return self._matvec_split(theta, theta.get_leg_labels())
             return super().matvec(theta)
-
-    # the device-optimised contraction routes of the engine's own TwoSiteH (everything but the constructor and the
-    # environment updates, which stay the reference's): methods and their class-level switches, by name prefix
-    take = ('_matvec_split', '_identity_env', '_dense_recipe', '_apply_W01', '_split_t2_views', '_use_split', 'deferred_check',
-            'identity_check', 'identity_env', 'mpo_apply', 'SPLIT_MIN_BLOCK', 'stats')
-    for name, val in vars(_EngineH).items():
-        if name.startswith(take) and name not in vars(B200TwoSiteH):
-            setattr(B200TwoSiteH, name, val)
 
     class B200TwoSiteDMRGEngine(ref_dmrg.TwoSiteDMRGEngine):
         EffectiveH = B200TwoSiteH

@@ -246,15 +246,18 @@ def test_svd_extensions_host_logic(fake_device):
 
 def test_matvec_split_order_equals_combined(fake_device):
     """`TwoSiteH.matvec` in the 'split' contraction order (LP, W0 W1, RP on the split theta; d times fewer flops)
-    returns the same Array as the reference's combined sequence LHeff . theta . RHeff -- dense, U(1) and U(1)xU(1)"""
+    returns the same Array as the reference's combined sequence LHeff . theta . RHeff -- dense, U(1) and U(1)xU(1), and
+    dense with K = D d^2 = 96 > 32, where W0 W1 is applied by npc.tensordot instead of the streaming kernel"""
     from tenpy_b200.models import TFIChain, SpinChain, FermiHubbardChain
     from tenpy_b200.networks.mps import MPS
     from tenpy_b200.algorithms import dmrg
     from tenpy_b200.algorithms.mps_common import TwoSiteH
     from tenpy_b200.linalg import np_conserved as npc
+    dense_hubbard = FermiHubbardChain({'L': 6, 't': 1., 'U': 4., 'mu': 0., 'cons_N': None, 'cons_Sz': None})
     cases = [(TFIChain({'L': 8, 'J': 1., 'g': 1.1, 'conserve': None}), ['up'] * 8, None),
              (SpinChain({'L': 8, 'Jx': 1., 'Jy': 1., 'Jz': 0.7, 'conserve': 'Sz'}), ['up', 'down'] * 4, True),
-             (FermiHubbardChain({'L': 6, 't': 1., 'U': 4., 'mu': 0.}), ['up', 'down'] * 3, True)]
+             (FermiHubbardChain({'L': 6, 't': 1., 'U': 4., 'mu': 0.}), ['up', 'down'] * 3, True),
+             (dense_hubbard, ['up', 'down'] * 3, None)]
     for M, state, mixer in cases:
         psi = MPS.from_product_state(M.lat_sites, state)
         eng = dmrg.TwoSiteDMRGEngine(psi, M, {'mixer': mixer, 'combine': True, 'matvec_order': 'combined',
@@ -265,9 +268,12 @@ def test_matvec_split_order_equals_combined(fake_device):
         for i0 in range(L - 1):
             Hc = TwoSiteH(eng.env, i0, combine=True, matvec_order='combined')
             Hs = TwoSiteH(eng.env, i0, combine=True, matvec_order='split')
-            Hs.identity_env = False      # the contraction order alone (the identity shortcut: test_matvec_identity_env)
+            Hs.identity_env = False      # the contraction order alone (the identity shortcut: test_matvec_identity_env_routes)
             theta = Hc.combine_theta(psi.get_theta(i0, 2))
+            n_mid = fake_device.calls.get('mid_contract', 0)
             a, b = Hc.matvec(theta), Hs.matvec(theta)
+            if M is dense_hubbard:
+                assert fake_device.calls.get('mid_contract', 0) == n_mid
             assert a.get_leg_labels() == b.get_leg_labels()
             assert npc.norm(a - b) <= 1e-13 * max(npc.norm(a), 1e-300)
         # 'auto' picks the combined order for these small blocks, and 'split' once the threshold is lowered
@@ -297,9 +303,9 @@ def test_dmrg_driver_split_matvec(fake_device):
     assert np.max(np.abs(psi.entanglement_entropy() - g['xxz_S'])) < 1e-7
 
 
-def test_matvec_fused_mpo_apply(fake_device):
-    """split-order matvec with `mpo_apply='fused'` (b200_mid_contract_f64: W0.W1 applied to the middle legs in one
-    streaming pass) equals the tensordot route; only taken for dense (one block) tensors"""
+def test_matvec_fused_mid_contract(fake_device):
+    """split-order matvec on dense (one block) tensors with K = D d^2 <= 32: W0.W1 is applied to the middle legs by
+    b200_mid_contract_f64 in one streaming pass; equals LP . theta . (W0 W1) . RP contracted by npc.tensordot"""
     from tenpy_b200.models import TFIChain, SpinChain
     from tenpy_b200.networks.mps import MPS
     from tenpy_b200.algorithms import dmrg
@@ -311,25 +317,28 @@ def test_matvec_fused_mpo_apply(fake_device):
     eng.sweep()
     eng.sweep()
     for i0 in range(7):
-        Ht = TwoSiteH(eng.env, i0, combine=True, matvec_order='split')
         Hf = TwoSiteH(eng.env, i0, combine=True, matvec_order='split')
-        Ht.identity_env = Hf.identity_env = False      # b200_mid_contract_f64 (the two-segment kernel: identity test)
-        Ht.mpo_apply, Hf.mpo_apply = 'tensordot', 'fused'
-        theta = Ht.combine_theta(psi.get_theta(i0, 2))
+        Hf.identity_env = False      # b200_mid_contract_f64 (the two-segment kernel: identity test)
+        theta = Hf.combine_theta(psi.get_theta(i0, 2))
+        a = npc.tensordot(Hf.LP, theta.split_legs(['(vL.p0)', '(p1.vR)']), axes=['vR', 'vL'])
+        a = npc.tensordot(a, npc.tensordot(Hf.W0, Hf.W1, axes=['wR', 'wL']),
+                          axes=[['wR', 'p0', 'p1'], ['wL', 'p0*', 'p1*']])
+        a = npc.tensordot(a, Hf.RP, axes=[['vR', 'wR'], ['vL', 'wL']]).ireplace_labels(['vR*', 'vL*'], ['vL', 'vR'])
+        a = a.combine_legs([['vL', 'p0'], ['p1', 'vR']], pipes=[Hf.pipeL, Hf.pipeR]).itranspose(theta.get_leg_labels())
         n0 = fake_device.calls.get('mid_contract', 0)
-        a, b = Ht.matvec(theta), Hf.matvec(theta)
+        b = Hf.matvec(theta)
         assert fake_device.calls.get('mid_contract', 0) == n0 + 1
         assert a.get_leg_labels() == b.get_leg_labels()
         assert npc.norm(a - b) <= 1e-13 * max(npc.norm(a), 1e-300)
-    # whole run with the option; with charges the fused route silently falls back to tensordot
+    # whole runs: dense, and with charges, where the streaming kernel is never taken
     g = h.load('dmrg.npz')
     M = TFIChain({'L': 20, 'J': 1., 'g': 1., 'conserve': None})
     res, psi = _run_dmrg(M, ['up'] * 20, {'mixer': None, 'max_E_err': 1e-10, 'combine': True, 'matvec_order': 'split',
-                                         'mpo_apply': 'fused', 'trunc_params': {'chi_max': 50, 'svd_min': 1e-10}})
+                                         'trunc_params': {'chi_max': 50, 'svd_min': 1e-10}})
     assert abs(res['E'] - g['tfi_E']) < 1e-10 * abs(g['tfi_E'])
     M = SpinChain({'L': 8, 'Jx': 1., 'Jy': 1., 'Jz': 1., 'conserve': 'Sz'})
     n0 = fake_device.calls.get('mid_contract', 0)
-    _run_dmrg(M, ['up', 'down'] * 4, {'mixer': True, 'matvec_order': 'split', 'mpo_apply': 'fused', 'max_sweeps': 3,
+    _run_dmrg(M, ['up', 'down'] * 4, {'mixer': True, 'matvec_order': 'split', 'max_sweeps': 3,
                                      'trunc_params': {'chi_max': 16, 'svd_min': 1e-10}})
     assert fake_device.calls.get('mid_contract', 0) == n0
 
@@ -520,10 +529,11 @@ def test_split_matvec_shares_buffers_without_charges(fake_device):
         assert theta.split_legs(['(vL.p0)', '(p1.vR)'], _view=True)._buf.data_ptr() != theta._buf.data_ptr()
 
 
-def test_matvec_identity_env(fake_device):
+def test_matvec_identity_env_routes(fake_device):
     """split-order matvec with `identity_env=True`: the identity components LP[IdL], RP[IdR] of the environments are
-    skipped (D-1 instead of D large GEMMs per side); same result on canonical states (dense, U(1), U(1)xU(1)); falls back
-    when the environment component is not the identity"""
+    skipped (D-1 instead of D large GEMMs per side); same result on canonical states (dense, U(1), U(1)xU(1), and dense
+    with K1 + K2 = D d^2 = 96 > 32, where W0 W1 is applied by npc.tensordot); falls back when the environment component is
+    not the identity"""
     from tenpy_b200.models import TFIChain, SpinChain, FermiHubbardChain
     from tenpy_b200.networks.mps import MPS
     from tenpy_b200.algorithms import dmrg
@@ -531,7 +541,9 @@ def test_matvec_identity_env(fake_device):
     from tenpy_b200.linalg import np_conserved as npc
     cases = [(TFIChain({'L': 8, 'J': 1., 'g': 1.1, 'conserve': None}), ['up'] * 8, None),
              (SpinChain({'L': 8, 'Jx': 1., 'Jy': 1., 'Jz': 0.7, 'conserve': 'Sz'}), ['up', 'down'] * 4, True),
-             (FermiHubbardChain({'L': 6, 't': 1., 'U': 4., 'mu': 0.}), ['up', 'down'] * 3, True)]
+             (FermiHubbardChain({'L': 6, 't': 1., 'U': 4., 'mu': 0.}), ['up', 'down'] * 3, True),
+             (FermiHubbardChain({'L': 6, 't': 1., 'U': 4., 'mu': 0., 'cons_N': None, 'cons_Sz': None}), ['up', 'down'] * 3,
+              None)]
     for M, state, mixer in cases:
         psi = MPS.from_product_state(M.lat_sites, state)
         eng = dmrg.TwoSiteDMRGEngine(psi, M, {'mixer': mixer, 'combine': True, 'matvec_order': 'combined',
@@ -545,14 +557,13 @@ def test_matvec_identity_env(fake_device):
         for i0 in range(psi.L - 1):
             Hc = TwoSiteH(eng.env, i0, combine=True, matvec_order='combined')
             Hi = TwoSiteH(eng.env, i0, combine=True, matvec_order='split')
-            Hi.identity_env, Hi.mpo_apply = True, 'tensordot'      # the tensordot route (the fused kernel is tested below)
+            Hi.identity_env = True
             theta = Hc.combine_theta(psi.get_theta(i0, 2))
             a, b = Hc.matvec(theta), Hi.matvec(theta)
             if mixer is None and Hi._id_env:      # no charges: the two components of t2 are shared views, nothing is gathered
                 n_take = fake_device.calls.get('take_blocks', 0)
-                c = Hi.matvec(theta)     # second call: GEMM 1 writes straight into the packed [LP_rest.theta, theta]
+                c = Hi.matvec(theta)     # TFI: the replayed kernel sequence; dense Hubbard (K1 + K2 > 32): W0 W1 by tensordot
                 assert fake_device.calls.get('take_blocks', 0) == n_take
-                assert getattr(Hi, '_t1_cat', None) is not None
                 assert npc.norm(c - b) <= 1e-14 * max(npc.norm(b), 1e-300)
             used += int(bool(Hi._id_env))
             assert a.get_leg_labels() == b.get_leg_labels()
@@ -569,7 +580,7 @@ def test_matvec_identity_env(fake_device):
     for i0 in range(1, psi0.L - 2):
         Hc = TwoSiteH(eng0.env, i0, combine=True, matvec_order='combined')
         Hf = TwoSiteH(eng0.env, i0, combine=True, matvec_order='split')
-        Hf.identity_env, Hf.mpo_apply = True, 'fused'
+        Hf.identity_env = True
         theta = Hc.combine_theta(psi0.get_theta(i0, 2))
         n0 = fake_device.calls.get('mid_contract2', 0)
         a, b = Hc.matvec(theta), Hf.matvec(theta)
