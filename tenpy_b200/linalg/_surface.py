@@ -85,8 +85,8 @@ def array_getitem(self, inds):
         res = res.copy(deep=True)
         res.iproject(masks, proj_axes)
         for a, order in zip(proj_axes, perms):
-            if order is not None:
-                res = res.permute(np.argsort(order), a)
+            if order is not None:      # the projection keeps the indices sorted: entry i is the order[i]-th of them
+                res = res.permute(order, a)
     if int_axes:
         res = res.take_slice([int(inds[a]) + (self.shape[a] if inds[a] < 0 else 0) for a in int_axes], int_axes)
     return res
@@ -100,6 +100,8 @@ def array_setitem(self, inds, other):
     inds = _normalize_inds(self, inds)
     dense = self.to_ndarray()
     val = other.to_ndarray() if isinstance(other, npc.Array) else other
+    if np.iscomplexobj(val) and not np.iscomplexobj(dense):
+        raise TypeError('a real Array can not hold complex values: assign to a ComplexArray (a.astype(complex))')
     np_inds = tuple(int(i) if isinstance(i, (int, np.integer)) else (i if isinstance(i, slice) else np.asarray(i))
                     for i in inds)
     dense[np_inds] = val
@@ -584,9 +586,7 @@ def _finish_complex(npc):
             a, b = self.re.get_block(qindices), self.im.get_block(qindices)
             if a is None and b is None:
                 return None
-            if a is None:
-                return 1.j * b
-            return a + (0. if b is None else 1.j * b)
+            return (0. if a is None else a) + 1.j * (0. if b is None else b)
 
         def test_sanity(self):
             self.re.test_sanity()
@@ -689,6 +689,28 @@ def _finish_complex(npc):
         def norm(self, ord=None, convert_to_float=True):
             return float(np.hypot(self.re.norm(ord), self.im.norm(ord)))
 
+        def scale_axis(self, s, axis=-1):
+            return self.copy(deep=True).iscale_axis(s, axis)
+
+        def iscale_axis(self, s, axis=-1):
+            """``(re + i im) (sr + i si)`` slice by slice along `axis`"""
+            s = np.asarray(s)
+            if np.iscomplexobj(s) and np.any(s.imag != 0.):
+                sr, si = np.ascontiguousarray(s.real), np.ascontiguousarray(s.imag)
+                re = self.re.scale_axis(sr, axis) - self.im.scale_axis(si, axis)
+                self.im = self.re.scale_axis(si, axis) + self.im.scale_axis(sr, axis)
+                self.re = re
+            else:
+                self.re.iscale_axis(s.real, axis)
+                self.im.iscale_axis(s.real, axis)
+            return self._sync()
+
+        def iproject(self, mask, axes):
+            self.im.iproject(mask, axes)
+            out = self.re.iproject(mask, axes)
+            self._sync()
+            return out
+
     # methods that act on both parts in the same way and return `self` / a new tensor
     def _inplace(name):
         def f(self, *args, **kwargs):
@@ -703,30 +725,32 @@ def _finish_complex(npc):
             return self._pair(getattr(self.re, name)(*args, **kwargs), getattr(self.im, name)(*args, **kwargs))
         f.__name__ = name
         return f
-    for name in ('iset_leg_labels', 'ireplace_label', 'ireplace_labels', 'idrop_labels', 'itranspose', 'iscale_axis',
-                 'iproject', 'iswapaxes', 'isort_qdata'):
+    for name in ('iset_leg_labels', 'ireplace_label', 'ireplace_labels', 'idrop_labels', 'itranspose', 'iswapaxes',
+                 'isort_qdata'):
         setattr(_ComplexArray, name, _inplace(name))
-    for name in ('transpose', 'replace_label', 'replace_labels', 'scale_axis', 'combine_legs', 'split_legs', 'take_slice',
-                 'add_leg', 'extend', 'add_trivial_leg', 'squeeze', 'gauge_total_charge'):
+    for name in ('transpose', 'replace_label', 'replace_labels', 'combine_legs', 'split_legs', 'take_slice', 'add_leg',
+                 'extend', 'add_trivial_leg', 'squeeze', 'gauge_total_charge'):
         setattr(_ComplexArray, name, _outofplace(name))
+    # public as np_conserved.ComplexArray: pickle finds the class there (this module's `ComplexArray` is the placeholder)
     _ComplexArray.__name__ = _ComplexArray.__qualname__ = 'ComplexArray'
+    _ComplexArray.__module__ = npc.__name__
     return _ComplexArray
 
 
-def complex_tensordot(npc, a, b, axes):
-    """tensordot with at least one ComplexArray operand from real contractions"""
+def complex_product(npc, a, b, prod):
+    """the bilinear product ``prod`` (tensordot, outer) with at least one ComplexArray operand, from the real products
+    of the parts"""
     CA = npc.ComplexArray
     a_re, a_im = (a.re, a.im) if isinstance(a, CA) else (a, None)
     b_re, b_im = (b.re, b.im) if isinstance(b, CA) else (b, None)
-    re = npc.tensordot(a_re, b_re, axes)
+    re = prod(a_re, b_re)
     if a_im is not None and b_im is not None:
-        t = npc.tensordot(a_im, b_im, axes)
-        re = re - t if isinstance(re, npc.Array) else re - t
+        re = re - prod(a_im, b_im)
     im = None
     if b_im is not None:
-        im = npc.tensordot(a_re, b_im, axes)
+        im = prod(a_re, b_im)
     if a_im is not None:
-        t = npc.tensordot(a_im, b_re, axes)
+        t = prod(a_im, b_re)
         im = t if im is None else im + t
     if not isinstance(re, npc.Array):          # full contraction: scalars
         return complex(re, im)

@@ -94,6 +94,9 @@ class _WriteThroughBlock(np.ndarray):
     _target = None
 
     def __setitem__(self, key, value):
+        if np.iscomplexobj(value):
+            raise TypeError('a block of a real Array can not hold complex values: assign to the blocks of a '
+                            'ComplexArray (.re / .im)')
         np.ndarray.__setitem__(self, key, value)
         if self._target is not None:
             buf, o, s = self._target
@@ -322,7 +325,8 @@ class Array:
     @classmethod
     def from_func(cls, func, legcharges, dtype=None, qtotal=None, func_args=(), func_kwargs={}, shape_kw=None,
                   labels=None):
-        """Fill all charge-allowed blocks with ``func(shape)`` (reference npc:617)."""
+        """Fill all charge-allowed blocks with ``func(shape)`` (reference npc:617).  Complex blocks give a
+        :class:`ComplexArray`, as in :meth:`from_blocks`."""
         legcharges = list(legcharges)
         chinfo = legcharges[0].chinfo
         qd = _allowed_qindices(legcharges, qtotal, chinfo)
@@ -335,7 +339,8 @@ class Array:
                 kw = dict(func_kwargs)
                 kw[shape_kw] = shape
                 blk = func(*func_args, **kw)
-            blocks.append(np.asarray(blk, dtype=np.float64).reshape(shape))
+            blk = np.asarray(blk)
+            blocks.append((blk if np.iscomplexobj(blk) else blk.astype(np.float64, copy=False)).reshape(shape))
         return cls.from_blocks(legcharges, qd, blocks, qtotal, labels)
 
     def zeros_like(self):
@@ -518,7 +523,12 @@ class Array:
         return self
 
     def iadd_prefactor_other(self, prefactor, other):
-        """``self += prefactor * other`` (reference npc:2373 / pyx:860)."""
+        """``self += prefactor * other`` (reference npc:2373 / pyx:860).  A real Array can not become complex in place:
+        a complex `prefactor` or a :class:`ComplexArray` `other` raises TypeError (``self + prefactor * other`` gives
+        the ComplexArray)."""
+        if isinstance(other, ComplexArray) or isinstance(prefactor, (complex, np.complexfloating)):
+            raise TypeError('iadd_prefactor_other of a real Array with a complex prefactor or a ComplexArray: use the '
+                            'out-of-place form self + prefactor * other')
         if self.rank != other.rank or self.shape != other.shape:
             raise ValueError('incompatible shapes {0} vs {1}'.format(self.shape, other.shape))
         if np.any(self.qtotal != other.qtotal):
@@ -621,14 +631,24 @@ class Array:
         return float(np.sqrt(backend.read_scalar(out)))
 
     def astype(self, dtype, copy=True):
+        """float64: a copy; complex128: a :class:`ComplexArray` with this Array as real part and no imaginary blocks."""
+        if np.dtype(dtype) == np.complex128:
+            return ComplexArray(self.copy(deep=True), self.zeros_like())
         if np.dtype(dtype) != np.float64:
-            raise NotImplementedError('float64 only')
+            raise NotImplementedError('Arrays are float64 or complex128 (ComplexArray), not {0}'.format(np.dtype(dtype)))
         return self.copy(deep=copy)
 
     # ------------------------------------------------------------------ scale_axis / project
     def iscale_axis(self, s, axis=-1):
-        """Multiply slice ``i`` along `axis` by ``s[i]`` (reference npc:2108)."""
+        """Multiply slice ``i`` along `axis` by ``s[i]`` (reference npc:2108).  A real Array can not become complex in
+        place: `s` with a non-zero imaginary part raises TypeError (:meth:`scale_axis` returns the ComplexArray)."""
         axis = self.get_leg_index(axis)
+        if np.iscomplexobj(s):
+            s = np.asarray(s)
+            if np.any(s.imag != 0.):
+                raise TypeError('iscale_axis of a real Array with complex factors: use scale_axis, which returns a '
+                                'ComplexArray')
+            s = s.real
         s = np.asarray(s, dtype=np.float64)
         if s.shape != (self.shape[axis],):
             raise ValueError('s has wrong shape {0}, expected ({1},)'.format(s.shape, self.shape[axis]))
@@ -646,6 +666,10 @@ class Array:
         return self
 
     def scale_axis(self, s, axis=-1):
+        """Copy of `self` with slice ``i`` along `axis` multiplied by ``s[i]``; complex `s` gives a ComplexArray."""
+        if np.iscomplexobj(s):
+            s = np.asarray(s)
+            return ComplexArray(self.scale_axis(s.real, axis), self.scale_axis(s.imag, axis))
         return self.copy(deep=True).iscale_axis(s, axis)
 
     def iproject(self, mask, axes):
@@ -1049,8 +1073,12 @@ def detect_qtotal(flat_array, legcharges, cutoff=None):
 
 def concatenate(arrays, axis=0, copy=True):
     """Stack Arrays along `axis` like ``np.concatenate`` (reference npc:3027): the leg is the concatenation of the
-    legs (neither sorted nor bunched), every stored block stays a block; labels from the first array."""
+    legs (neither sorted nor bunched), every stored block stays a block; labels from the first array.  With a
+    :class:`ComplexArray` among `arrays` the real and the imaginary parts are concatenated separately."""
     arrays = list(arrays)
+    if any(isinstance(a, ComplexArray) for a in arrays):
+        parts = [(a.re, a.im) if isinstance(a, ComplexArray) else (a, a.zeros_like()) for a in arrays]
+        return ComplexArray(concatenate([p[0] for p in parts], axis, copy), concatenate([p[1] for p in parts], axis, copy))
     first = arrays[0]
     axis = first.get_leg_index(axis)
     not_axis = [a for a in range(first.rank) if a != axis]
@@ -1095,7 +1123,11 @@ def concatenate(arrays, axis=0, copy=True):
 
 
 def diag(s, leg, dtype=None, labels=None):
-    """2D Array with `s` on the diagonal, legs ``(leg, leg.conj())`` (reference npc:3234)."""
+    """2D Array with `s` on the diagonal, legs ``(leg, leg.conj())`` (reference npc:3234); a ComplexArray for complex
+    `s`."""
+    if np.iscomplexobj(s):
+        s = np.asarray(s)
+        return ComplexArray(diag(s.real, leg, labels=labels), diag(s.imag, leg, labels=labels))
     s = np.asarray(s, dtype=np.float64)
     scalar = s.ndim == 0
     if not scalar and s.shape != (leg.ind_len,):
@@ -1150,7 +1182,7 @@ def tensordot(a, b, axes=2, _out=None, _oz_slices=None):
     size without alignment padding, written instead of a fresh allocation (lets a caller place the result inside a
     larger packed buffer)."""
     if isinstance(a, ComplexArray) or isinstance(b, ComplexArray):
-        return _sf.complex_tensordot(_sys.modules[__name__], a, b, axes)
+        return _sf.complex_product(_sys.modules[__name__], a, b, lambda x, y: tensordot(x, y, axes))
     a, b, n = _prepare_contraction(a, b, axes)
     cut_a = a.rank - n
     if cut_a == 0 and b.rank == n:
@@ -1287,6 +1319,8 @@ def _labels_unique(labels):
 
 def outer(a, b):
     """Outer product (reference npc:3575), via a contraction over zero legs."""
+    if isinstance(a, ComplexArray) or isinstance(b, ComplexArray):
+        return _sf.complex_product(_sys.modules[__name__], a, b, outer)
     a2, b2, n = _prepare_contraction(a, b, 0)
     res_legs = a.legs + b.legs
     labels = a._labels + b._labels
