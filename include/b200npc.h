@@ -297,6 +297,18 @@ int b200_block_eigh_f64(int64_t nblocks, const int64_t *n_host, const int64_t *a
                         const int64_t *w_off_host, const int64_t *v_off_host, const double *A, double *W,
                         double *V, void *work_dev, int64_t work_bytes, int32_t *info_host,
                         b200_stream_t stream);
+/* Complex counterpart of b200_block_eigh_f64: A_i = V_i diag(W_i) V_i^H for complex Hermitian row-major blocks, with the
+ * same shapes, offsets, synchronous call, info_host, sweep limit and error codes.  PLANAR data: A_re / A_im and V_re /
+ * V_im are separate f64 buffers that share one offset table (a_off[i], v_off[i]); W_i is real and ascending, V_i unitary
+ * with the eigenvectors in its COLUMNS: A_i V_i = V_i diag(W_i).  The iteration sees (A_i + A_i^H) / 2, as a Hermitian
+ * solver reading one triangle would.  Range: every finite block.  The iteration runs on 2^-e A_i, 2^e the power of two of
+ * max |a_ij| over the real and imaginary parts (exact): V is bit for bit that of 2^-e A_i, W exactly 2^e times its W
+ * (rounded once where it is subnormal).  Accuracy |A_i|_F-normwise.
+ * replaces _eig_worker npc:5041 (np.linalg.eigh, LAPACK zheevd) for complex blocks. */
+int64_t b200_block_eigh_z_worksize(int64_t nblocks, const int64_t *n_host);
+int b200_block_eigh_z(int64_t nblocks, const int64_t *n_host, const int64_t *a_off_host, const int64_t *w_off_host,
+                      const int64_t *v_off_host, const double *A_re, const double *A_im, double *W, double *V_re,
+                      double *V_im, void *work_dev, int64_t work_bytes, int32_t *info_host, b200_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -89,6 +89,9 @@ _SIGNATURES = {
     'b200_block_eigh_worksize': (c_i64, [c_i64, c_i64p]),
     'b200_block_eigh_f64': (ctypes.c_int, [c_i64, c_i64p, c_i64p, c_i64p, c_i64p, c_vp, c_vp, c_vp, c_vp, c_i64,
                                            c_i32p, c_vp]),
+    'b200_block_eigh_z_worksize': (c_i64, [c_i64, c_i64p]),
+    'b200_block_eigh_z': (ctypes.c_int, [c_i64, c_i64p, c_i64p, c_i64p, c_i64p, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                         c_i64, c_i32p, c_vp]),
 }
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))
 
@@ -467,16 +470,26 @@ class DeviceLib:
         other values leave it unchanged (complex rounds always use jacobi_eig_kernel<true>); returns the old value"""
         return int(self.c.b200_svd_set_eig_variant(int(variant)))
 
-    def block_eigh(self, n, a_off, w_off, v_off, A, W, V):
+    def _eigh_call(self, fn, worksize, prof, n, a_off, w_off, v_off, A, W, V):
+        """one batched block eigh through `fn` (b200_block_eigh_f64 or b200_block_eigh_z); A, V: tuples of planes"""
         ns, ao, wo, vo = [_i64(x) for x in (n, a_off, w_off, v_off)]
         nb = len(ns[0])
-        wbytes = int(self.c.b200_block_eigh_worksize(nb, ns[1]))
+        wbytes = int(worksize(nb, ns[1]))
         work = self.torch.empty(wbytes, dtype=self.torch.uint8, device=self.device)
         info = np.zeros(nb, dtype=np.int32)
-        with _Prof(self, 'eigh'):
-            self._check(self.c.b200_block_eigh_f64(nb, ns[1], ao[1], wo[1], vo[1], _ptr(A), _ptr(W), _ptr(V),
-                                                   _ptr(work), wbytes, info.ctypes.data_as(c_i32p), self.stream()))
+        with _Prof(self, prof):
+            self._check(fn(nb, ns[1], ao[1], wo[1], vo[1], *map(_ptr, A + (W,) + V), _ptr(work), wbytes,
+                           info.ctypes.data_as(c_i32p), self.stream()))
         return info
+
+    def block_eigh(self, n, a_off, w_off, v_off, A, W, V):
+        return self._eigh_call(self.c.b200_block_eigh_f64, self.c.b200_block_eigh_worksize, 'eigh', n, a_off, w_off,
+                               v_off, (A,), W, (V,))
+
+    def block_eigh_z(self, n, a_off, w_off, v_off, A_re, A_im, W, V_re, V_im):
+        """complex Hermitian block eigh on planar buffers (include/b200npc.h): W real ascending, V unitary; returns info"""
+        return self._eigh_call(self.c.b200_block_eigh_z, self.c.b200_block_eigh_z_worksize, 'eigh_z', n, a_off, w_off,
+                               v_off, (A_re, A_im), W, (V_re, V_im))
 
     def kernel_launch_count(self, reset=False):
         return int(self.c.b200_kernel_launch_count(1 if reset else 0))

@@ -87,7 +87,8 @@ def full_diag_effH(effH, theta_guess, keep_sector=True):
     pipe = theta_guess.make_pipe(effH.acts_on, qconj=+1)
     fullH.legs[0].test_equal(pipe)
     qi = pipe.get_qindex_of_charges(theta_guess.qtotal)
-    if not np.any(fullH._qdata[:, 0] == qi):
+    parts = (fullH.re, fullH.im) if isinstance(fullH, npc.ComplexArray) else (fullH,)
+    if not any(np.any(part._qdata[:, 0] == qi) for part in parts):
         logger.warning('H is zero in the given block, nothing to diagonalize. We just return the initial state.')
         return 0., theta_guess
     W, V = npc.eigh(fullH)
@@ -415,6 +416,8 @@ class TwoSiteDMRGEngine:
         """Reference dmrg.py:672: Lanczos, or for ``diag_method='default'`` and tiny effective Hamiltonians
         (``N < max_N_for_ED``) the exact diagonalisation of the charge block (`full_diag_effH`)."""
         N = -1
+        if self.eff_H.dtype is not np.float64 and not isinstance(theta_guess, npc.ComplexArray):
+            theta_guess = theta_guess.astype(np.complex128)       # a real state, a complex Hamiltonian
         if self.diag_method == 'ED_block' or (self.diag_method == 'default' and
                                               self.eff_H.N < self.options.get('max_N_for_ED', 400)):
             E, theta = full_diag_effH(self.eff_H, theta_guess, keep_sector=True)
@@ -430,7 +433,8 @@ class TwoSiteDMRGEngine:
                 self._pending_scalars.append(('norm2', None, n2))
         # overlap of the new with the old wave function: a statistic only -- computed on the device now, read with all the
         # others at the end of the sweep (no host round trip between the Lanczos result and the SVD)
-        if theta_guess._layout.nblocks and theta_guess._layout.same_blocks(theta._layout) and \
+        if not isinstance(theta, npc.ComplexArray) and not isinstance(theta_guess, npc.ComplexArray) and \
+                theta_guess._layout.nblocks and theta_guess._layout.same_blocks(theta._layout) and \
                 theta_guess.get_leg_labels() == theta.get_leg_labels() and np.all(theta_guess.qtotal == theta.qtotal):
             lib = backend.get_lib()
             ov = backend.empty(1)
@@ -503,7 +507,7 @@ class TwoSiteDMRGEngine:
         i0 = self.i0
         E_trunc = None
         if self._meas_E_trunc or E0 is None:
-            E_trunc = float(self.env.full_contraction(self._update_env_inds()[0]))    # uses the updated LP / RP
+            E_trunc = float(np.real(self.env.full_contraction(self._update_env_inds()[0])))   # uses the updated LP / RP
             if E0 is None:
                 E0 = E_trunc
             E_trunc = E_trunc - E0

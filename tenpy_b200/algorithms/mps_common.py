@@ -583,9 +583,11 @@ class TwoSiteH(SplitOrderMatvec):
             self.combine_Heff(env)
 
     def matvec(self, theta):
-        """Apply the effective Hamiltonian to `theta` (reference mps_common.py:1321)."""
+        """Apply the effective Hamiltonian to `theta` (reference mps_common.py:1321).  A complex `theta` or MPO takes the
+        combined (or plain) order: the split-order routes and their per-bond caches are real-only."""
         labels = theta.get_leg_labels()
-        if self.combine and self._use_split(theta):
+        if self.combine and self.dtype is np.float64 and not isinstance(theta, npc.ComplexArray) and \
+                self._use_split(theta):
             return self._matvec_split(theta, labels)
         chain, relabel = _TWO_SITE_CHAINS['combined' if self.combine else 'plain']
         return _apply_chain(self, theta, chain, relabel).itranspose(labels)

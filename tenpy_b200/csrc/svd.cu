@@ -2,7 +2,7 @@
 //
 // Replaces, on the GPU, the per-charge-block LAPACK calls of the reference:
 //   npc._svd_worker (tenpy/linalg/np_conserved.py:4950) -> svd_robust.svd (svd_robust.py:37, gesdd/gesvd)
-//   npc._eig_worker (np_conserved.py:5041)              -> np.linalg.eigh (syevd)
+//   npc._eig_worker (np_conserved.py:5041)              -> np.linalg.eigh (syevd; zheevd for complex Hermitian blocks)
 //
 // Algorithm (all blocks of one Array in one batch):
 //   Each matrix is held as Y (q x p, q <= p, row-major, rows = the vectors to orthogonalise; Y = A or A^T)
@@ -813,7 +813,10 @@ __global__ void __launch_bounds__(256) svd_init_kernel(double *__restrict__ work
 }
 
 // eigh init: Y = scale * A + shift*I.  scale[mat] and shift[mat] are set by eigh_shift_kernel (after jacobi_amax_kernel).
-__global__ void __launch_bounds__(256) eigh_shift_kernel(JMat *__restrict__ mats, const double *__restrict__ A) {
+// CPLX: Ai is the imaginary plane of a Hermitian A; the norm is over both planes and amax (jacobi_amax_kernel) covers both
+template <bool CPLX>
+__global__ void __launch_bounds__(256) eigh_shift_kernel(JMat *__restrict__ mats, const double *__restrict__ A,
+                                                         const double *__restrict__ Ai) {
     __shared__ double red[32];
     JMat *mt = mats + blockIdx.x;
     const double *a = A + mt->a_off;
@@ -823,6 +826,10 @@ __global__ void __launch_bounds__(256) eigh_shift_kernel(JMat *__restrict__ mats
     for (int64_t e = threadIdx.x; e < nn; e += blockDim.x) {
         const double x = a[e] * scale;
         s = fma(x, x, s);
+        if constexpr (CPLX) {
+            const double y = Ai[mt->a_off + e] * scale;
+            s = fma(y, y, s);
+        }
     }
     s = block_sum(s, red);
     // (no absolute term: the scaled block has max |a| in [1, 2), and a zero block needs no shift -- W = 0 exactly)
@@ -832,8 +839,10 @@ __global__ void __launch_bounds__(256) eigh_shift_kernel(JMat *__restrict__ mats
     }
 }
 
+// CPLX: Y = scale * (A + A^H) / 2 + shift*I -- the real plane symmetrised, the imaginary plane (Yi) antisymmetrised
+template <bool CPLX>
 __global__ void __launch_bounds__(256) eigh_init_kernel(double *__restrict__ work, const JMat *__restrict__ mats,
-                                                        const double *__restrict__ A) {
+                                                        const double *__restrict__ A, const double *__restrict__ Ai) {
     const JMat mt = mats[blockIdx.y];
     double *Y = work + mt.y_off;
     double *W = work + mt.w_off;
@@ -846,6 +855,11 @@ __global__ void __launch_bounds__(256) eigh_init_kernel(double *__restrict__ wor
         double v = 0.5 * (a[(int64_t)r * mt.n + c] * mt.scale + a[(int64_t)c * mt.n + r] * mt.scale);
         if (r == c) v += mt.shift;
         Y[(int64_t)r * mt.ldy + c] = v;
+        if constexpr (CPLX) {
+            const double *ai = Ai + mt.a_off;
+            work[mt.yi_off + (int64_t)r * mt.ldy + c] =
+                0.5 * (ai[(int64_t)r * mt.n + c] * mt.scale - ai[(int64_t)c * mt.n + r] * mt.scale);
+        }
     }
     for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < mt.qp; e += stride)
         W[e * mt.ldw + e] = 1.0;
@@ -1009,9 +1023,12 @@ __global__ void __launch_bounds__(128)
 }
 
 // eigh finalize: eigenvalue r (ascending) = (norm[perm[r]] - shift) / scale; V[:, r] = W[perm[r], :]
+// CPLX: W Y0 = Y with W unitary and the rows of Y orthogonal, so W Y0^2 W^H is diagonal and the eigenvectors of Y0 are the
+// columns of W^H: V[:, r] = conj(W[perm[r], :]) (svd_finalize_kernel writes Ui = -wi for the same reason)
+template <bool CPLX>
 __global__ void __launch_bounds__(128)
     eigh_finalize_kernel(const double *__restrict__ work, const JMat *__restrict__ mats, const int *__restrict__ perm,
-                         double *__restrict__ Wout, double *__restrict__ V) {
+                         double *__restrict__ Wout, double *__restrict__ V, double *__restrict__ Vi) {
     const JMat mt = mats[blockIdx.y];
     const int r = blockIdx.x;
     const int n = mt.n;
@@ -1021,6 +1038,11 @@ __global__ void __launch_bounds__(128)
     if (threadIdx.x == 0) Wout[mt.s_off + r] = (work[mt.snorm_off + src] - mt.shift) / mt.scale;
     double *v = V + mt.vt_off;
     for (int i = threadIdx.x; i < n; i += blockDim.x) v[(int64_t)i * n + r] = w[i];
+    if constexpr (CPLX) {
+        const double *wi = work + mt.wi_off + (int64_t)src * mt.ldw;
+        double *vi = Vi + mt.vt_off;
+        for (int i = threadIdx.x; i < n; i += blockDim.x) vi[(int64_t)i * n + r] = -wi[i];
+    }
 }
 
 // ---- host driver -----------------------------------------------------------------------------------
@@ -1532,14 +1554,16 @@ extern "C" int64_t b200_block_eigh_worksize(int64_t nblocks, const int64_t *n) {
     return L.total_bytes;
 }
 
-extern "C" int b200_block_eigh_f64(int64_t nblocks, const int64_t *n, const int64_t *a_off, const int64_t *w_off,
-                                   const int64_t *v_off, const double *A, double *Wout, double *V, void *work_dev,
-                                   int64_t work_bytes, int32_t *info, b200_stream_t stream) {
+// real (Ai == NULL) and complex Hermitian (planar: A + i Ai -> V + i Vi, W real) block eigh: one host driver
+static int block_eigh_impl(int64_t nblocks, const int64_t *n, const int64_t *a_off, const int64_t *w_off,
+                           const int64_t *v_off, const double *A, const double *Ai, double *Wout, double *V, double *Vi,
+                           void *work_dev, int64_t work_bytes, int32_t *info, b200_stream_t stream) {
     if (nblocks <= 0) return B200_OK;
     if (nblocks > 65535) return set_error(B200_ERR_ARG, "too many blocks for one eigh batch");
+    const bool cplx = Ai != nullptr;
     cudaStream_t st = (cudaStream_t)stream;
     JLayout L;
-    make_layout(nblocks, n, n, true, L);
+    make_layout(nblocks, n, n, true, L, cplx);
     if (work_bytes < L.total_bytes) return set_error(B200_ERR_ARG, "eigh work buffer too small");
     for (int64_t i = 0; i < nblocks; ++i) {
         if (n[i] <= 0) return set_error(B200_ERR_ARG, "empty block in eigh batch");
@@ -1556,27 +1580,60 @@ extern "C" int b200_block_eigh_f64(int64_t nblocks, const int64_t *n, const int6
     B200_CUDA_CHECK(cudaMemcpyAsync(work + L.off_cta, L.cta_mat.data(), L.cta_mat.size() * 4, cudaMemcpyHostToDevice, st));
     JMat *d_mats = reinterpret_cast<JMat *>(work + L.off_mats);
     double *wf = reinterpret_cast<double *>(work);
-    launch_amax(L.mats, d_mats, A, nullptr, st);
+    launch_amax(L.mats, d_mats, A, Ai, st);
     B200_CHECK_LAUNCH();
-    eigh_shift_kernel<<<nmat, 256, 0, st>>>(d_mats, A);
+    if (cplx)
+        eigh_shift_kernel<true><<<nmat, 256, 0, st>>>(d_mats, A, Ai);
+    else
+        eigh_shift_kernel<false><<<nmat, 256, 0, st>>>(d_mats, A, nullptr);
     B200_CHECK_LAUNCH();
     {
         int64_t max_elems = 0;
         for (auto &mt : L.mats) max_elems = std::max<int64_t>(max_elems, (int64_t)mt.q * mt.p);
         int64_t gx = std::min<int64_t>(std::max<int64_t>(1, (max_elems + 1023) / 1024), 2048);
-        eigh_init_kernel<<<dim3((unsigned)gx, (unsigned)nmat), 256, 0, st>>>(wf, d_mats, A);
+        if (cplx)
+            eigh_init_kernel<true><<<dim3((unsigned)gx, (unsigned)nmat), 256, 0, st>>>(wf, d_mats, A, Ai);
+        else
+            eigh_init_kernel<false><<<dim3((unsigned)gx, (unsigned)nmat), 256, 0, st>>>(wf, d_mats, A, nullptr);
         B200_CHECK_LAUNCH();
     }
-    int rc = run_jacobi(L, work, st, info, 40);
+    int rc = run_jacobi(L, work, st, info, 40, cplx);
     if (rc) return rc;
     std::vector<int> perm;
     rc = sort_norms(L, work, st, true, perm);
     if (rc) return rc;
-    eigh_finalize_kernel<<<dim3((unsigned)std::max(1, L.max_q), (unsigned)nmat), 128, 0, st>>>(
-        wf, d_mats, reinterpret_cast<int *>(work + L.off_perm), Wout, V);
+    const dim3 fgrid((unsigned)std::max(1, L.max_q), (unsigned)nmat);
+    int *d_perm = reinterpret_cast<int *>(work + L.off_perm);
+    if (cplx)
+        eigh_finalize_kernel<true><<<fgrid, 128, 0, st>>>(wf, d_mats, d_perm, Wout, V, Vi);
+    else
+        eigh_finalize_kernel<false><<<fgrid, 128, 0, st>>>(wf, d_mats, d_perm, Wout, V, nullptr);
     B200_CHECK_LAUNCH();
     B200_CUDA_CHECK(cudaStreamSynchronize(st));
     for (int i = 0; i < nmat; ++i)
         if (info[i] < 0) return set_error(B200_ERR_NOCONV, "block Jacobi eigh did not converge for block %d", i);
     return B200_OK;
+}
+
+extern "C" int b200_block_eigh_f64(int64_t nblocks, const int64_t *n, const int64_t *a_off, const int64_t *w_off,
+                                   const int64_t *v_off, const double *A, double *Wout, double *V, void *work_dev,
+                                   int64_t work_bytes, int32_t *info, b200_stream_t stream) {
+    return block_eigh_impl(nblocks, n, a_off, w_off, v_off, A, nullptr, Wout, V, nullptr, work_dev, work_bytes, info,
+                           stream);
+}
+
+extern "C" int64_t b200_block_eigh_z_worksize(int64_t nblocks, const int64_t *n) {
+    if (nblocks <= 0) return 256;
+    JLayout L;
+    make_layout(nblocks, n, n, true, L, true);
+    return L.total_bytes;
+}
+
+extern "C" int b200_block_eigh_z(int64_t nblocks, const int64_t *n, const int64_t *a_off, const int64_t *w_off,
+                                 const int64_t *v_off, const double *A_re, const double *A_im, double *W, double *V_re,
+                                 double *V_im, void *work_dev, int64_t work_bytes, int32_t *info, b200_stream_t stream) {
+    if (nblocks > 0 && (A_re == nullptr || A_im == nullptr || V_im == nullptr))
+        return set_error(B200_ERR_ARG, "complex eigh: both planes of A and V are needed");
+    return block_eigh_impl(nblocks, n, a_off, w_off, v_off, A_re, A_im, W, V_re, V_im, work_dev, work_bytes, info,
+                           stream);
 }

@@ -516,6 +516,20 @@ class ComplexArray:
     # the methods are attached in _finish_complex (they need np_conserved.Array)
 
 
+class _ComplexBlock(np.ndarray):
+    """host copy of one block of a ComplexArray; assignments are written through to the blocks of both parts"""
+    _parts = None
+
+    def __setitem__(self, key, value):
+        np.ndarray.__setitem__(self, key, value)
+        if self._parts is not None:
+            self._parts[0][...] = self.real
+            self._parts[1][...] = self.imag
+
+    def __array_finalize__(self, obj):
+        self._parts = None            # views / results of arithmetic are plain host data
+
+
 def _finish_complex(npc):
     Array = npc.Array
 
@@ -583,10 +597,18 @@ def _finish_complex(npc):
             raise NotImplementedError('block access of a ComplexArray: use .re / .im')
 
         def get_block(self, qindices, insert=False, raise_incomp_q=False):
-            a, b = self.re.get_block(qindices), self.im.get_block(qindices)
+            """the block as a complex host array, or None; stored in both parts (``insert=True`` stores zero blocks
+            first), item assignments are written through to both device buffers (``block[:] = values`` as in the
+            reference's ``full_diag_effH``, dmrg.py:1209)"""
+            a = self.re.get_block(qindices, insert, raise_incomp_q)
+            b = self.im.get_block(qindices, insert, raise_incomp_q)
             if a is None and b is None:
                 return None
-            return (0. if a is None else a) + 1.j * (0. if b is None else b)
+            if a is None or b is None:
+                return (0. if a is None else np.asarray(a)) + 1.j * (0. if b is None else np.asarray(b))
+            blk = (np.asarray(a) + 1.j * np.asarray(b)).view(_ComplexBlock)
+            blk._parts = (a, b)
+            return blk
 
         def test_sanity(self):
             self.re.test_sanity()

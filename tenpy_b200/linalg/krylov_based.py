@@ -23,6 +23,37 @@ __all__ = ['KrylovBased', 'LanczosGroundState', 'lanczos']
 DEVICE_SCALARS_DEFAULT = True    # Lanczos option `device_scalars`: (alpha, beta) stay on the device, read back in chunks
 
 
+def _pack(v, lay=None):
+    """A complex Krylov vector on the device-scalar route: the ComplexArray `v` with both parts in ONE device buffer
+    ``[re | im]`` of ``2 lay.size`` elements on the block table `lay` (default: the union of the tables of its parts).
+    For a Hermitian operator every step of the recurrence is a real operation on that buffer: ``alpha = Re<v|Hv>`` is the
+    real dot product of the packed planes, and the update, the normalisation and the result assembly have real
+    coefficients.  Returns the ComplexArray whose parts are views of the two halves, with the buffer as ``_kbuf``, or
+    ``None`` if the table of `v` differs from `lay`."""
+    union, re, im = npc._complex_planes(v)
+    if lay is None:
+        lay = union
+    elif not (union is lay or union.same_blocks(lay)):
+        return None
+    n = lay.size
+    buf = backend.empty(2 * n)
+    buf[:n].copy_(re)
+    buf[n:].copy_(im)
+    parts = [npc.Array(v.legs, np.float64, v.qtotal, v.get_leg_labels())._set_blocks(lay, half)
+             for half in (buf[:n], buf[n:])]
+    out = npc.ComplexArray(*parts)
+    out._kbuf = buf
+    return out
+
+
+def _flat(v):
+    """``(n, buffer)``: the real Array `v`, or the packed ComplexArray (:func:`_pack`), as one real device vector"""
+    kbuf = getattr(v, '_kbuf', None)
+    if kbuf is not None:
+        return kbuf.numel(), kbuf
+    return v._layout.size, v._buf
+
+
 class KrylovBased:
     """Base class: option parsing, cache and result assembly (reference krylov_based.py:30)."""
 
@@ -59,19 +90,24 @@ class KrylovBased:
         vf = self._result_krylov
         assert N == len(vf) > 1
         psif = self.psi0 * vf[0]
+        if not isinstance(psif, npc.ComplexArray) and any(isinstance(c, npc.ComplexArray) for c in self._cache):
+            psif = psif.astype(np.complex128)        # a real start vector, a complex operator
         len_cache = len(self._cache)
         for k in range(1, min(len_cache + 1, N)):
             psif.iadd_prefactor_other(vf[N - k], self._cache[-k])
         self._cache = []
         self._rebuild_krylov_for_result_full(psif, N - len_cache - 1)
-        if getattr(self, 'device_scalars', False) and psif._layout.nblocks:
+        if getattr(self, 'device_scalars', False) and isinstance(psif, npc.ComplexArray):
+            psif = _pack(psif)
+        if getattr(self, 'device_scalars', False) and _flat(psif)[0]:
             # normalisation without a host round trip (same arithmetic: |psi|^2 by the dot kernel, x *= 1 / sqrt(.)); the
             # conditioning warning of the reference is raised when somebody reads `norm_check()` (the DMRG engine: at the
             # end of the sweep)
             lib = backend.get_lib()
             n2 = backend.empty(1)
-            lib.dot(psif._layout.size, psif._buf, psif._buf, backend.dot_scratch(), n2)
-            lib.scal_rsqrt_dev(psif._layout.size, n2, psif._buf)
+            size, buf = _flat(psif)
+            lib.dot(size, buf, buf, backend.dot_scratch(), n2)
+            lib.scal_rsqrt_dev(size, n2, buf)
             self._result_norm2_dev = n2
             return psif
         psif_norm = npc.norm(psif)
@@ -126,33 +162,43 @@ class LanczosGroundState(KrylovBased):
         vectors do not share one block layout (caller falls back to the host-scalar loop)."""
         h = self._h_krylov
         lib = backend.get_lib()
+        cplx = isinstance(self.psi0, npc.ComplexArray)
+        if cplx:
+            self.psi0 = _pack(self.psi0)          # normalised in place below, like a real start vector
         w = self.psi0
-        if w._layout.nblocks == 0:
+        lay = w.re._layout if cplx else w._layout
+        if lay.nblocks == 0:
             raise ValueError('Norm of self.psi0 too small: 0.0')
+        size = _flat(w)[0]
         # sc[2k] = alpha_k, sc[2k+1] = |w_k|^2 = beta_{k+1}^2; last entry: |psi0|^2 -- the start vector is normalised on the
         # device as well (same arithmetic as `npc.norm` + `iscale_prefactor`), its norm is tested with the first chunk of
         # scalars: no host round trip before the first `N_min` matvecs are enqueued
         sc = backend.zeros(2 * self.N_max + 1)
         nrm2_0 = sc[2 * self.N_max:2 * self.N_max + 1]
         scratch = backend.dot_scratch()
-        lib.dot(w._layout.size, w._buf, w._buf, scratch, nrm2_0)
+        lib.dot(size, _flat(w)[1], _flat(w)[1], scratch, nrm2_0)
         done_k = 0                                     # iterations whose scalars have been processed on the host
         k = 0
         while k < self.N_max:
             stop_at = self.N_min if k < self.N_min else min(self.N_max, k + self.sync_every)
             while k < stop_at:
-                lib.scal_rsqrt_dev(w._layout.size, nrm2_0 if k == 0 else sc[2 * k - 1:2 * k], w._buf)
+                lib.scal_rsqrt_dev(size, nrm2_0 if k == 0 else sc[2 * k - 1:2 * k], _flat(w)[1])
                 self._to_cache(w)
                 w = self.H.matvec(w)
                 v1 = self._cache[-1]
-                if not (w._layout is v1._layout or w._layout.same_blocks(v1._layout)):
+                if cplx:
+                    w = _pack(w if isinstance(w, npc.ComplexArray) else w.astype(np.complex128), lay)
+                elif isinstance(w, npc.ComplexArray) or not (w._layout is v1._layout or
+                                                             w._layout.same_blocks(v1._layout)):
+                    w = None                                  # (a real start vector, a complex operator: host loop)
+                if w is None:
                     if self._psi0_norm is None:
                         self._psi0_norm = float(np.sqrt(backend.read_scalar(nrm2_0)))
                     return None
-                lib.dot(w._layout.size, w._buf, v1._buf, scratch, sc[2 * k:2 * k + 1])
-                v0 = self._cache[-2]._buf if k > 0 else None
-                lib.lanczos_update_dev(w._layout.size, sc[2 * k:2 * k + 1], v1._buf,
-                                       sc[2 * k - 1:2 * k] if k > 0 else None, v0, w._buf, scratch,
+                lib.dot(size, _flat(w)[1], _flat(v1)[1], scratch, sc[2 * k:2 * k + 1])
+                v0 = _flat(self._cache[-2])[1] if k > 0 else None
+                lib.lanczos_update_dev(size, sc[2 * k:2 * k + 1], _flat(v1)[1],
+                                       sc[2 * k - 1:2 * k] if k > 0 else None, v0, _flat(w)[1], scratch,
                                        sc[2 * k + 1:2 * k + 2])
                 k += 1
             vals = backend.to_host(sc)                                # the one synchronisation of this chunk
@@ -202,12 +248,14 @@ class LanczosGroundState(KrylovBased):
             w.iscale_prefactor(1. / beta)
             self._to_cache(w)
             w = self.H.matvec(w)
-            alpha = float(npc.inner(w, self._cache[-1], axes='range', do_conj=True))
+            # (Re: a ComplexArray gives a complex inner product, real up to rounding for a Hermitian H)
+            alpha = float(np.real(npc.inner(w, self._cache[-1], axes='range', do_conj=True)))
             if k == 0 and getattr(self.H, 'deferred_check', None) is not None:
                 self.H.deferred_check()                                # tests the operator postponed to its first read-back
             h[k, k] = alpha
             self._calc_result_krylov(k)
-            fused = (not self.reortho) and w._layout.same_blocks(self._cache[-1]._layout) and \
+            fused = (not self.reortho) and not isinstance(w, npc.ComplexArray) and \
+                w._layout.same_blocks(self._cache[-1]._layout) and \
                 (k == 0 or w._layout.same_blocks(self._cache[-2]._layout))
             if fused:
                 # w -= alpha v_k + beta v_{k-1};  beta' = |w|   in ONE pass (b200_lanczos_update_f64)

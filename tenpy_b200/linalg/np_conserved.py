@@ -120,6 +120,29 @@ class Array:
     `size`; plus `_layout` (the :class:`BlockLayout`) and `_buf` (the device buffer).
     """
 
+    _dtype = _F64
+
+    @property
+    def dtype(self):
+        return self._dtype
+
+    @dtype.setter
+    def dtype(self, dtype):
+        """Assigning complex128 to a real Array makes it a :class:`ComplexArray` in place (its blocks become the real
+        part), as the reference promotes an Array whose dtype is set (``theta.dtype = ...`` in its ``full_diag_effH``,
+        dmrg.py:1207, before complex values are written into a block)."""
+        dtype = np.dtype(dtype)
+        if dtype.kind == 'c' and not isinstance(self, ComplexArray):
+            re = Array.__new__(Array)
+            re.__dict__.update(self.__dict__)
+            self.__dict__.clear()
+            self.__class__ = ComplexArray
+            ComplexArray.__init__(self, re, re.zeros_like())
+        elif (dtype.kind == 'c') != isinstance(self, ComplexArray):
+            raise TypeError('dtype {0} for a ComplexArray: use astype()'.format(dtype))
+        else:
+            self._dtype = dtype
+
     def __init__(self, legcharges, dtype=np.float64, qtotal=None, labels=None):
         self.legs = legs = list(legcharges)
         self.rank = rank = len(legs)
@@ -1345,8 +1368,8 @@ def inner(a, b, axes='labels', do_conj=False):
 
     `axes`: ``'range'`` = leg k of `a` with leg k of `b`; ``'labels'`` (default) = match by label (conjugated
     labels for ``do_conj=False``); or ``(axes_a, axes_b)``.  ``do_conj=True`` conjugates `a` first.
-    With a :class:`ComplexArray` operand the result is a Python ``complex``, composed of the real inner products of the
-    parts."""
+    With a :class:`ComplexArray` operand the result is a ``np.complex128`` (a Python ``complex``), composed of the real
+    inner products of the parts."""
     if isinstance(a, list) and isinstance(b, list):
         return sum(inner(w, v, axes=axes, do_conj=do_conj) for w, v in zip(a, b))
     if isinstance(a, ComplexArray) or isinstance(b, ComplexArray):
@@ -1358,7 +1381,7 @@ def inner(a, b, axes='labels', do_conj=False):
             return 0. if x is None or y is None else float(inner(x, y, axes=axes, do_conj=do_conj))
         re = part(a_re, b_re) + sgn * part(a_im, b_im)
         im = part(a_re, b_im) - sgn * part(a_im, b_re)
-        return complex(re, im)
+        return np.complex128(complex(re, im))        # (a numpy scalar, like the reference's: np.real(..).item() works)
     if a.rank != b.rank:
         raise ValueError('different rank!')
     if axes != 'range':
@@ -2001,23 +2024,47 @@ def eigvalsh(a, UPLO='L', sort=None):
     return eigh(a, UPLO, sort)[0]
 
 
+def _hermitian_defect(a):
+    """``(|a - a^H|_F^2, |a|_F^2)`` of the square ComplexArray `a`: four dot products on the device, one read back"""
+    d = a - a.conj().itranspose()
+    lib = backend.get_lib()
+    out = backend.zeros(4)
+    for j, part in enumerate((d.re, d.im, a.re, a.im)):
+        lay = part._layout
+        if lay.nblocks:
+            lib.dot(lay.size, part._buf, part._buf, backend.dot_scratch(), out[j:j + 1])
+    r = backend.to_host(out)
+    return float(r[0] + r[1]), float(r[2] + r[3])
+
+
 def eigh(a, UPLO='L', sort=None):
     """Eigen-decomposition of a hermitian 2D Array with contractible legs (reference npc:3899 / :5041).
 
     Returns ``(W, V)``: eigenvalues (1D host array, ordered like the first leg; within a block ascending or
     as requested by `sort`) and the unitary `V` with legs ``(a.legs[0], a.legs[0].conj() as LegCharge)``.
-    Missing diagonal blocks give eigenvalue 0 with unit vectors, exactly like the reference."""
-    if isinstance(a, ComplexArray):
-        raise NotImplementedError('eigh of a complex Hermitian matrix is not implemented (only real symmetric blocks)')
+    Missing diagonal blocks give eigenvalue 0 with unit vectors, exactly like the reference.
+    A :class:`ComplexArray` `a` must be Hermitian to ``|a - a^H|_F <= 1e-8 |a|_F`` (else NotImplementedError: only
+    Hermitian eigenproblems are provided); it goes through the complex block-Jacobi kernel (``b200_block_eigh_z``), `W`
+    is real and `V` a ComplexArray."""
+    cplx = isinstance(a, ComplexArray)
     if a.rank != 2 or a.shape[0] != a.shape[1]:
         raise ValueError('expect a square matrix!')
     a.legs[0].test_contractible(a.legs[1])
     if np.any(a.qtotal != a.chinfo.make_valid()):
         raise ValueError('Non-trivial qtotal -> Nilpotent. Not diagonizable!?')
+    if cplx:
+        defect2, norm2 = _hermitian_defect(a)
+        if not defect2 <= 1e-16 * norm2:
+            raise NotImplementedError('eigh: the ComplexArray is not complex Hermitian (|A - A^H|_F = {0:.3g} |A|_F); '
+                                      'only Hermitian eigenproblems are provided'.format(
+                                          np.sqrt(defect2 / norm2) if norm2 > 0. else np.inf))
     a_label0 = a._labels[0]
     piped_axes, a = a.as_completely_blocked()
     leg = a.legs[0]
-    lay = a._layout
+    if cplx:
+        lay, bufA, bufA_im = _complex_planes(a)
+    else:
+        lay, bufA = a._layout, a._buf
     if np.any(lay.qdata[:, 0] != lay.qdata[:, 1]):
         raise ValueError('off-diagonal blocks in a completely blocked matrix with zero charge?')
     resw = np.zeros(a.shape[0], dtype=np.float64)
@@ -2039,19 +2086,25 @@ def eigh(a, UPLO='L', sort=None):
         bufV = backend.to_device(host)
     else:
         bufV = backend.zeros(lay_V.size)
+    planes = [bufV]
+    if cplx:
+        planes.append(backend.zeros(lay_V.size))
     if lay.nblocks:
         lib = backend.get_lib()
         nn = sizes[stored]
         w_off = np.concatenate(([0], np.cumsum(nn)))
         bufW = backend.empty(int(w_off[-1]))
-        lib.block_eigh(nn, lay.offsets, w_off[:-1], lay_V.offsets[stored], a._buf, bufW, bufV)
+        if cplx:
+            lib.block_eigh_z(nn, lay.offsets, w_off[:-1], lay_V.offsets[stored], bufA, bufA_im, bufW, bufV, planes[1])
+        else:
+            lib.block_eigh(nn, lay.offsets, w_off[:-1], lay_V.offsets[stored], bufA, bufW, bufV)
         w = backend.to_host(bufW)
         recs, pool, at = [], [], 0
         for j, qi in enumerate(stored):
             rw = w[w_off[j]:w_off[j + 1]]
             if sort is not None and sort != '<':
                 # order inside the block as requested (reference tools/misc.py argsort): permute the eigenvalues
-                # on the host and the columns of V with one take launch
+                # on the host and the columns of V with one take launch (per plane)
                 key = {'m<': np.abs(rw), 'm>': -np.abs(rw), '>': -rw}.get(sort)
                 if key is None:
                     raise ValueError('unknown sort option ' + repr(sort))
@@ -2065,9 +2118,15 @@ def eigh(a, UPLO='L', sort=None):
             resw[leg.get_slice(qi)] = rw
         if recs:
             rec = np.array(recs, dtype=np.int64)
-            src = bufV.clone()
-            lib.take_blocks(rec, backend.to_device(rec), backend.to_device(np.concatenate(pool)), src, bufV)
+            rec_dev, pool_dev = backend.to_device(rec), backend.to_device(np.concatenate(pool))
+            for buf in planes:
+                src = buf.clone()
+                lib.take_blocks(rec, rec_dev, pool_dev, src, buf)
     V._set_blocks(lay_V, bufV)
+    if cplx:
+        V_im = Array(V.legs, np.float64, None)
+        V_im._set_blocks(lay_V, planes[1])
+        V = ComplexArray(V, V_im)
     if len(piped_axes) > 0:
         V = V.split_legs(0)
     V.iset_leg_labels([a_label0, 'eig'] if a_label0 != 'eig' else [None, 'eig'])

@@ -7,7 +7,7 @@ down directly as its finite-state-machine MPO.  The resulting bond dimensions eq
 (TFI D=3, XXZ D=5, Hubbard D=6) and energies are pinned against the reference in tests/golden.
 
 * TFIChain:          ``H = -J sum_i sx_i sx_{i+1} - g sum_i sz_i``  (Pauli matrices)
-* SpinChain (S=1/2): ``H = sum_i Jx Sx Sx + Jy Sy Sy + Jz Sz Sz - hz sum_i Sz_i``
+* SpinChain (S=1/2): ``H = sum_i Jx Sx Sx + Jy Sy Sy + Jz Sz Sz + D (Sx Sy - Sy Sx) - hz sum_i Sz_i``
 * FermiHubbardChain: ``H = -t sum_{i,s} (c^+_{i,s} c_{i+1,s} + h.c.) + U sum_i n_up n_dn - mu sum_i n_i``
 """
 # Copyright (C) 2026 tenpy_b200 authors. Apache-2.0.
@@ -108,7 +108,11 @@ class TFIChain(_ChainModel):
 
 
 class SpinChain(_ChainModel):
-    """Spin-1/2 chain (reference spins.py `SpinChain`, S=0.5); params ``L, Jx, Jy, Jz, hz, conserve``."""
+    """Spin-1/2 chain (reference spins.py `SpinChain`, S=0.5); params ``L, Jx, Jy, Jz, hz, D, conserve``.
+
+    `D`: z-axis Dzyaloshinskii-Moriya coupling ``D sum_i (Sx_i Sy_{i+1} - Sy_i Sx_{i+1})
+    = (iD/2) sum_i (S+_i S-_{i+1} - S-_i S+_{i+1})``; it conserves Sz when ``Jx == Jy``.  A non-zero `D` makes the MPO
+    complex (ComplexArray tensors); with ``D = 0`` it is the real MPO."""
 
     def __init__(self, params):
         L = params['L']
@@ -116,6 +120,7 @@ class SpinChain(_ChainModel):
             raise NotImplementedError('S=1/2 only')
         Jx, Jy, Jz = params.get('Jx', 1.), params.get('Jy', 1.), params.get('Jz', 1.)
         hz = params.get('hz', 0.)
+        D = params.get('D', 0.)
         conserve = params.get('conserve', 'best')
         if conserve == 'best':
             conserve = 'Sz' if Jx == Jy else 'parity'
@@ -124,9 +129,10 @@ class SpinChain(_ChainModel):
         site = SpinHalfSite(conserve=conserve)
         jpm = (Jx + Jy) / 4.
         jpp = (Jx - Jy) / 4.
+        dm = 0.5j * D          # S+_i S-_{i+1} gets +iD/2, S-_i S+_{i+1} gets -iD/2
         last = [[(-hz, 'Sz')] if hz != 0. else None,
-                [(jpm, 'Sm')] + ([(jpp, 'Sp')] if jpp != 0. else []),
-                [(jpm, 'Sp')] + ([(jpp, 'Sm')] if jpp != 0. else []),
+                [(jpm + dm if D != 0. else jpm, 'Sm')] + ([(jpp, 'Sp')] if jpp != 0. else []),
+                [(jpm - dm if D != 0. else jpm, 'Sp')] + ([(jpp, 'Sm')] if jpp != 0. else []),
                 [(Jz, 'Sz')],
                 [(1., 'Id')]]
         grid = [[[(1., 'Id')], [(1., 'Sp')], [(1., 'Sm')], [(1., 'Sz')], last[0]],

@@ -24,7 +24,6 @@ class MPO:
         self.L = len(self.sites)
         self.bc = bc
         self.finite = True
-        self.dtype = np.float64
         self.chinfo = self.sites[0].leg.chinfo
         self._W = [W.itranspose(['wL', 'wR', 'p', 'p*']) for W in Ws]
         self.IdL = list(IdL) if isinstance(IdL, (list, tuple)) else [IdL] * (self.L + 1)
@@ -37,13 +36,18 @@ class MPO:
 
         grids[i][a][b] is ``None`` or a list of ``(coefficient, opname)``; `w_charges` is a list (length
         L+1) of (D, qnumber) charge tables of the MPO bonds (``None`` for no charges).  The MPO legs are
-        *not bunched*: every MPO index is its own charge sector, like the reference's MPO legs."""
+        *not bunched*: every MPO index is its own charge sector, like the reference's MPO legs.
+        Complex coefficients or operators make every ``W`` a ComplexArray (if any of them has an imaginary part)."""
         sites = list(sites)
         chinfo = sites[0].leg.chinfo
+        cplx = any(np.iscomplexobj(coef) and coef.imag != 0. or np.iscomplexobj(site.get_dense(name))
+                   for site, grid in zip(sites, grids) for row in grid for entry in row if entry is not None
+                   for coef, name in entry)
+        W_cls = npc.ComplexArray if cplx else npc.Array
         Ws = []
         for i, (site, grid) in enumerate(zip(sites, grids)):
             D1, D2 = len(grid), len(grid[0])
-            dense = np.zeros((D1, D2, site.dim, site.dim))
+            dense = np.zeros((D1, D2, site.dim, site.dim), dtype=np.complex128 if cplx else np.float64)
             for a in range(D1):
                 for b in range(D2):
                     if grid[a][b] is None:
@@ -56,9 +60,14 @@ class MPO:
             else:
                 legL = LegCharge.from_qind(chinfo, np.arange(D1 + 1), w_charges[i], +1)
                 legR = LegCharge.from_qind(chinfo, np.arange(D2 + 1), w_charges[i + 1], -1)
-            Ws.append(npc.Array.from_ndarray(dense, [legL, legR, site.leg, site.leg.conj()],
-                                             labels=['wL', 'wR', 'p', 'p*'], qtotal=None, cutoff=1e-15))
+            Ws.append(W_cls.from_ndarray(dense, [legL, legR, site.leg, site.leg.conj()],
+                                         labels=['wL', 'wR', 'p', 'p*'], qtotal=None, cutoff=1e-15))
         return cls(sites, Ws, IdL, IdR)
+
+    @property
+    def dtype(self):
+        """complex128 if a tensor is a ComplexArray, else float64"""
+        return np.complex128 if any(isinstance(W, npc.ComplexArray) for W in self._W) else np.float64
 
     @property
     def chi(self):
@@ -86,12 +95,16 @@ class MPOEnvironment:
         self.bra, self.ket, self.H = bra, ket, H
         self.L = ket.L
         self.finite = True
-        self.dtype = np.float64
         self._LP = [None] * self.L
         self._RP = [None] * self.L
         self._LP_age = [None] * self.L
         self._RP_age = [None] * self.L
         self.init_first_LP_last_RP(**init_env_data)
+
+    @property
+    def dtype(self):
+        """complex128 if the MPO or one of the states is complex, else float64"""
+        return np.result_type(self.bra.dtype, self.H.dtype, self.ket.dtype).type
 
     def init_first_LP_last_RP(self, init_LP=None, init_RP=None, age_LP=0, age_RP=0):
         if init_LP is None:

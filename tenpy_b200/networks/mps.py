@@ -29,7 +29,6 @@ class MPS:
         self.bc = bc
         self.finite = True
         self.chinfo = self.sites[0].leg.chinfo
-        self.dtype = np.float64
         self.norm = norm
         self.form = [self._to_valid_form(form)] * self.L if not isinstance(form, list) else \
             [self._to_valid_form(f) for f in form]
@@ -37,6 +36,12 @@ class MPS:
         self._S = [None if s is None else np.array(s, dtype=np.float64) for s in SVs]
         if len(self._S) != self.L + 1:
             raise ValueError('need L+1 singular value arrays')
+
+    @property
+    def dtype(self):
+        """complex128 once a tensor is a ComplexArray (a product state is real; the first complex update makes it
+        complex), else float64"""
+        return np.complex128 if any(isinstance(B, npc.ComplexArray) for B in self._B) else np.float64
 
     def _to_valid_form(self, form):
         if isinstance(form, tuple):
@@ -237,7 +242,8 @@ class MPS:
             self.set_SL(i, S)
             self.set_B(i, V.split_legs(1), form='B')
         assert len(S) == 1
-        self._B[0] *= float(U.to_ndarray()[0, 0])             # a sign, kept like the reference does
+        u = U.to_ndarray()[0, 0]                               # a sign (a phase for a complex state), kept like the
+        self._B[0] *= u if isinstance(U, npc.ComplexArray) else float(u)      # reference does
 
     def _normalize_array(self, arr, renormalize):
         """Reference mps.py:6151."""

@@ -41,7 +41,9 @@ class Site:
             self.add_op('Id', np.eye(self.dim), permute=False)
 
     def add_op(self, name, op, permute=True):
-        op = np.asarray(op, dtype=np.float64)
+        """`op`: dense (d, d); real (float64) unless it has a non-zero imaginary part (complex128)"""
+        op = np.asarray(op)
+        op = op.astype(np.complex128 if np.iscomplexobj(op) and np.any(op.imag != 0.) else np.float64)
         if permute:
             op = op[np.ix_(self.perm, self.perm)]
         self._dense[name] = op
@@ -63,10 +65,10 @@ class Site:
         return dq[0]
 
     def get_op(self, name):
-        """device Array with labels ``'p', 'p*'``"""
+        """device Array (a ComplexArray for a complex operator) with labels ``'p', 'p*'``"""
         if name not in self._npc:
-            self._npc[name] = npc.Array.from_ndarray(self._dense[name], [self.leg, self.leg.conj()],
-                                                     labels=['p', 'p*'])
+            cls = npc.ComplexArray if np.iscomplexobj(self._dense[name]) else npc.Array
+            self._npc[name] = cls.from_ndarray(self._dense[name], [self.leg, self.leg.conj()], labels=['p', 'p*'])
         return self._npc[name]
 
     def state_index(self, label):
