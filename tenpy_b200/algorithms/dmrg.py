@@ -87,7 +87,7 @@ def full_diag_effH(effH, theta_guess, keep_sector=True):
     pipe = theta_guess.make_pipe(effH.acts_on, qconj=+1)
     fullH.legs[0].test_equal(pipe)
     qi = pipe.get_qindex_of_charges(theta_guess.qtotal)
-    parts = (fullH.re, fullH.im) if isinstance(fullH, npc.ComplexArray) else (fullH,)
+    parts = (fullH.re, fullH.im) if np.dtype(fullH.dtype).kind == 'c' else (fullH,)
     if not any(np.any(part._qdata[:, 0] == qi) for part in parts):
         logger.warning('H is zero in the given block, nothing to diagonalize. We just return the initial state.')
         return 0., theta_guess
@@ -416,7 +416,7 @@ class TwoSiteDMRGEngine:
         """Reference dmrg.py:672: Lanczos, or for ``diag_method='default'`` and tiny effective Hamiltonians
         (``N < max_N_for_ED``) the exact diagonalisation of the charge block (`full_diag_effH`)."""
         N = -1
-        if self.eff_H.dtype is not np.float64 and not isinstance(theta_guess, npc.ComplexArray):
+        if np.dtype(self.eff_H.dtype).kind == 'c' and np.dtype(theta_guess.dtype).kind != 'c':
             theta_guess = theta_guess.astype(np.complex128)       # a real state, a complex Hamiltonian
         if self.diag_method == 'ED_block' or (self.diag_method == 'default' and
                                               self.eff_H.N < self.options.get('max_N_for_ED', 400)):
@@ -433,7 +433,7 @@ class TwoSiteDMRGEngine:
                 self._pending_scalars.append(('norm2', None, n2))
         # overlap of the new with the old wave function: a statistic only -- computed on the device now, read with all the
         # others at the end of the sweep (no host round trip between the Lanczos result and the SVD)
-        if not isinstance(theta, npc.ComplexArray) and not isinstance(theta_guess, npc.ComplexArray) and \
+        if np.dtype(theta.dtype).kind != 'c' and np.dtype(theta_guess.dtype).kind != 'c' and \
                 theta_guess._layout.nblocks and theta_guess._layout.same_blocks(theta._layout) and \
                 theta_guess.get_leg_labels() == theta.get_leg_labels() and np.all(theta_guess.qtotal == theta.qtotal):
             lib = backend.get_lib()

@@ -586,7 +586,7 @@ class TwoSiteH(SplitOrderMatvec):
         """Apply the effective Hamiltonian to `theta` (reference mps_common.py:1321).  A complex `theta` or MPO takes the
         combined (or plain) order: the split-order routes and their per-bond caches are real-only."""
         labels = theta.get_leg_labels()
-        if self.combine and self.dtype is np.float64 and not isinstance(theta, npc.ComplexArray) and \
+        if self.combine and np.dtype(self.dtype).kind != 'c' and np.dtype(theta.dtype).kind != 'c' and \
                 self._use_split(theta):
             return self._matvec_split(theta, labels)
         chain, relabel = _TWO_SITE_CHAINS['combined' if self.combine else 'plain']

@@ -104,7 +104,6 @@ def fast_two_site_engine():
     from tenpy.algorithms import dmrg as ref_dmrg
     from tenpy.algorithms import mps_common as ref_common
     from .algorithms.mps_common import SplitOrderMatvec
-    from .linalg import np_conserved as npc
 
     class B200TwoSiteH(SplitOrderMatvec, ref_common.TwoSiteH):
         """reference ``TwoSiteH`` (same constructor, attributes, `combine_theta`, `update_LP` ...); `matvec` applies
@@ -117,7 +116,7 @@ def fast_two_site_engine():
 
         def matvec(self, theta):
             # the split-order routes are real-only: a complex theta or MPO takes the reference's order
-            if self.combine and np.dtype(self.dtype).kind != 'c' and not isinstance(theta, npc.ComplexArray) and \
+            if self.combine and np.dtype(self.dtype).kind != 'c' and np.dtype(theta.dtype).kind != 'c' and \
                     self._use_split(theta):
                 return self._matvec_split(theta, theta.get_leg_labels())
             return super().matvec(theta)

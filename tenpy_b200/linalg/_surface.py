@@ -4,20 +4,15 @@ states, indexing, sorting of leg charges, element-wise functions, small dense fa
 (model construction, measurements); they are implemented on top of the hot-path primitives of
 :mod:`tenpy_b200.linalg.np_conserved` (block moves, tensordot, eigh on the device) and, where the reference itself works
 element by element on the host (``from_ndarray``, ``__setitem__`` of a few numbers), by one host round trip of the small
-tensor involved.  Imported at the end of ``np_conserved.py``, which attaches the methods to :class:`Array`.
-
-`ComplexArray` gives complex128 tensors as a pair of real device Arrays (same legs, planar storage); elementwise operations,
-contractions and inner products are composed of the real kernels.  It carries the reference's `Site` operators (``Sy`` & co.)
-and real-time evolution: ``npc.svd`` and ``npc.qr`` of a ComplexArray run the complex block-Jacobi SVD and the complex
-Householder QR kernels (``b200_block_svd_z``, ``b200_block_qr_z``), so the reference's TEBD with ``exp(-i dt H)`` runs on
-the engine.  ``npc.eigh`` of a complex Hermitian matrix is not provided (NotImplementedError).
+tensor involved.  Imported at the end of ``np_conserved.py``, which attaches the methods to :class:`Array`.  Complex
+tensors (`ComplexArray`) are in :mod:`tenpy_b200.linalg._complex`.
 """
 import numpy as np
 
 from . import charges as _ch
 from .charges import LegCharge, LegPipe, QTYPE
 
-__all__ = ['QCUTOFF', 'ComplexArray', 'grid_outer', 'grid_concat', 'detect_grid_outer_legcharge', 'detect_legcharge', 'eig',
+__all__ = ['QCUTOFF', 'grid_outer', 'grid_concat', 'detect_grid_outer_legcharge', 'detect_legcharge', 'eig',
            'eigvals', 'speigs', 'expm', 'lq', 'polar', 'orthogonal_columns']
 
 QCUTOFF = np.finfo(np.float64).eps * 10.   # reference np_conserved.py:146
@@ -461,7 +456,7 @@ def expm(a):
             pass
     import scipy.linalg
     piped, b = a.as_completely_blocked()
-    if isinstance(b, npc.ComplexArray):       # (the class np_conserved attached, not the placeholder of this module)
+    if isinstance(b, npc.ComplexArray):
         dense = scipy.linalg.expm(b.to_ndarray())
         res = npc.ComplexArray.from_ndarray(dense, b.legs, qtotal=b.qtotal, cutoff=0., labels=b._labels)
     else:
@@ -506,274 +501,3 @@ def lq(a, mode='reduced', inner_labels=[None, None], cutoff=None, pos_diag_L=Fal
     Q, R = npc.qr(a.transpose(), mode=mode, inner_labels=[label_Q, label_L], cutoff=cutoff, pos_diag_R=pos_diag_L,
                   qtotal_Q=qtotal_Q, inner_qconj=-inner_qconj)
     return R.itranspose(), Q.itranspose()
-
-
-# ------------------------------------------------------------------------------------------------ complex tensors
-class ComplexArray:
-    """complex128 tensor = two real device Arrays ``re``, ``im`` on the same legs (see the module doc string); the class
-    is made a subclass of :class:`Array` by ``np_conserved`` when it attaches this module (``isinstance`` checks of the
-    reference hold)."""
-    # the methods are attached in _finish_complex (they need np_conserved.Array)
-
-
-class _ComplexBlock(np.ndarray):
-    """host copy of one block of a ComplexArray; assignments are written through to the blocks of both parts"""
-    _parts = None
-
-    def __setitem__(self, key, value):
-        np.ndarray.__setitem__(self, key, value)
-        if self._parts is not None:
-            self._parts[0][...] = self.real
-            self._parts[1][...] = self.imag
-
-    def __array_finalize__(self, obj):
-        self._parts = None            # views / results of arithmetic are plain host data
-
-
-def _finish_complex(npc):
-    Array = npc.Array
-
-    class _ComplexArray(Array):
-        __doc__ = ComplexArray.__doc__
-
-        def __init__(self, re, im):
-            self.re, self.im = re, im
-            self.legs = list(re.legs)
-            self._labels = list(re._labels)
-            self.rank, self.shape = re.rank, re.shape
-            self.dtype = np.dtype(np.complex128)
-            self.chinfo, self.qtotal = re.chinfo, re.qtotal
-            self._qdata_sorted = True
-
-        # ---- construction / conversion
-        @classmethod
-        def from_ndarray(cls, data_flat, legcharges, dtype=None, qtotal=None, cutoff=None, labels=None,
-                         raise_wrong_sector=True, warn_wrong_sector=True):
-            data_flat = np.asarray(data_flat, dtype=np.complex128)
-            legcharges = list(legcharges)
-            if qtotal is None:
-                qtotal = Array.detect_qtotal(data_flat, legcharges, cutoff)
-            kw = dict(qtotal=qtotal, cutoff=cutoff, labels=labels, raise_wrong_sector=raise_wrong_sector,
-                      warn_wrong_sector=warn_wrong_sector)
-            return cls(Array.from_ndarray(np.ascontiguousarray(data_flat.real), legcharges, **kw),
-                       Array.from_ndarray(np.ascontiguousarray(data_flat.imag), legcharges, **kw))
-
-        @classmethod
-        def from_blocks(cls, legcharges, qdata, blocks, qtotal=None, labels=None):
-            blocks = [np.asarray(b, dtype=np.complex128) for b in blocks]
-            return cls(Array.from_blocks(legcharges, qdata, [np.ascontiguousarray(b.real) for b in blocks], qtotal, labels),
-                       Array.from_blocks(legcharges, qdata, [np.ascontiguousarray(b.imag) for b in blocks], qtotal, labels))
-
-        def to_ndarray(self):
-            return self.re.to_ndarray() + 1.j * self.im.to_ndarray()
-
-        def _pair(self, re, im):
-            return _ComplexArray(re, im)
-
-        def copy(self, deep=True):
-            return self._pair(self.re.copy(deep), self.im.copy(deep))
-
-        def astype(self, dtype, copy=True):
-            if np.dtype(dtype).kind == 'c':
-                return self.copy(deep=True) if copy else self
-            if npc.norm(self.im) > 0.:
-                import warnings
-                warnings.warn('discarding the imaginary part', stacklevel=2)
-            return self.re.copy(deep=True)
-
-        @property
-        def stored_blocks(self):
-            return max(self.re.stored_blocks, self.im.stored_blocks)
-
-        @property
-        def size(self):
-            return self.re.size
-
-        @property
-        def _layout(self):
-            raise NotImplementedError('a ComplexArray has no single packed layout (real and imaginary part separately)')
-
-        def get_blocks_host(self):
-            raise NotImplementedError('block access of a ComplexArray: use .re / .im')
-
-        def get_block(self, qindices, insert=False, raise_incomp_q=False):
-            """the block as a complex host array, or None; stored in both parts (``insert=True`` stores zero blocks
-            first), item assignments are written through to both device buffers (``block[:] = values`` as in the
-            reference's ``full_diag_effH``, dmrg.py:1209)"""
-            a = self.re.get_block(qindices, insert, raise_incomp_q)
-            b = self.im.get_block(qindices, insert, raise_incomp_q)
-            if a is None and b is None:
-                return None
-            if a is None or b is None:
-                return (0. if a is None else np.asarray(a)) + 1.j * (0. if b is None else np.asarray(b))
-            blk = (np.asarray(a) + 1.j * np.asarray(b)).view(_ComplexBlock)
-            blk._parts = (a, b)
-            return blk
-
-        def test_sanity(self):
-            self.re.test_sanity()
-            self.im.test_sanity()
-
-        def zeros_like(self):
-            return self._pair(self.re.zeros_like(), self.im.zeros_like())
-
-        def __repr__(self):
-            return '<npc.ComplexArray shape={0!s} labels={1!s}>'.format(self.shape, self._labels)
-
-        def __getstate__(self):
-            return {'re': self.re, 'im': self.im}
-
-        def __setstate__(self, state):
-            self.__init__(state['re'], state['im'])
-
-        # ---- labels: keep both parts and the wrapper in step
-        def _sync(self):
-            self.legs = list(self.re.legs)
-            self._labels = list(self.re._labels)
-            self.rank, self.shape = self.re.rank, self.re.shape
-            self.qtotal = self.re.qtotal
-            return self
-
-        # ---- arithmetic
-        def iconj(self, complex_conj=True):
-            self.re.iconj()
-            self.im.iconj()
-            if complex_conj:
-                self.im.iscale_prefactor(-1.)
-            return self._sync()
-
-        def conj(self, complex_conj=True):
-            return self.copy(deep=True).iconj(complex_conj)
-
-        def complex_conj(self):
-            return self._pair(self.re.copy(deep=True), self.im * -1.)
-
-        def iscale_prefactor(self, prefactor):
-            z = complex(prefactor)
-            if z.imag == 0.:
-                self.re.iscale_prefactor(z.real)
-                self.im.iscale_prefactor(z.real)
-            else:
-                re = self.re * z.real - self.im * z.imag
-                im = self.re * z.imag + self.im * z.real
-                self.re, self.im = re, im
-            return self
-
-        def iadd_prefactor_other(self, prefactor, other):
-            z = complex(prefactor)
-            o_re, o_im = (other.re, other.im) if isinstance(other, _ComplexArray) else (other, None)
-            if z.real != 0.:
-                self.re.iadd_prefactor_other(z.real, o_re)
-                if o_im is not None:
-                    self.im.iadd_prefactor_other(z.real, o_im)
-            if z.imag != 0.:
-                self.im.iadd_prefactor_other(z.imag, o_re)
-                if o_im is not None:
-                    self.re.iadd_prefactor_other(-z.imag, o_im)
-            return self
-
-        def __mul__(self, other):
-            if np.isscalar(other):
-                return self.copy(deep=True).iscale_prefactor(other)
-            return NotImplemented
-
-        __rmul__ = __mul__
-
-        def __imul__(self, other):
-            return self.iscale_prefactor(other) if np.isscalar(other) else NotImplemented
-
-        def __truediv__(self, other):
-            return self.__mul__(1. / other) if np.isscalar(other) else NotImplemented
-
-        def __itruediv__(self, other):
-            return self.iscale_prefactor(1. / other) if np.isscalar(other) else NotImplemented
-
-        def __neg__(self):
-            return self.__mul__(-1.)
-
-        def __add__(self, other):
-            return self.copy(deep=True).iadd_prefactor_other(1., other) if isinstance(other, Array) else NotImplemented
-
-        __radd__ = __add__
-
-        def __iadd__(self, other):
-            return self.iadd_prefactor_other(1., other) if isinstance(other, Array) else NotImplemented
-
-        def __sub__(self, other):
-            return self.copy(deep=True).iadd_prefactor_other(-1., other) if isinstance(other, Array) else NotImplemented
-
-        def __rsub__(self, other):
-            return (self * -1.).iadd_prefactor_other(1., other) if isinstance(other, Array) else NotImplemented
-
-        def __isub__(self, other):
-            return self.iadd_prefactor_other(-1., other) if isinstance(other, Array) else NotImplemented
-
-        def norm(self, ord=None, convert_to_float=True):
-            return float(np.hypot(self.re.norm(ord), self.im.norm(ord)))
-
-        def scale_axis(self, s, axis=-1):
-            return self.copy(deep=True).iscale_axis(s, axis)
-
-        def iscale_axis(self, s, axis=-1):
-            """``(re + i im) (sr + i si)`` slice by slice along `axis`"""
-            s = np.asarray(s)
-            if np.iscomplexobj(s) and np.any(s.imag != 0.):
-                sr, si = np.ascontiguousarray(s.real), np.ascontiguousarray(s.imag)
-                re = self.re.scale_axis(sr, axis) - self.im.scale_axis(si, axis)
-                self.im = self.re.scale_axis(si, axis) + self.im.scale_axis(sr, axis)
-                self.re = re
-            else:
-                self.re.iscale_axis(s.real, axis)
-                self.im.iscale_axis(s.real, axis)
-            return self._sync()
-
-        def iproject(self, mask, axes):
-            self.im.iproject(mask, axes)
-            out = self.re.iproject(mask, axes)
-            self._sync()
-            return out
-
-    # methods that act on both parts in the same way and return `self` / a new tensor
-    def _inplace(name):
-        def f(self, *args, **kwargs):
-            getattr(self.re, name)(*args, **kwargs)
-            getattr(self.im, name)(*args, **kwargs)
-            return self._sync()
-        f.__name__ = name
-        return f
-
-    def _outofplace(name):
-        def f(self, *args, **kwargs):
-            return self._pair(getattr(self.re, name)(*args, **kwargs), getattr(self.im, name)(*args, **kwargs))
-        f.__name__ = name
-        return f
-    for name in ('iset_leg_labels', 'ireplace_label', 'ireplace_labels', 'idrop_labels', 'itranspose', 'iswapaxes',
-                 'isort_qdata'):
-        setattr(_ComplexArray, name, _inplace(name))
-    for name in ('transpose', 'replace_label', 'replace_labels', 'combine_legs', 'split_legs', 'take_slice', 'add_leg',
-                 'extend', 'add_trivial_leg', 'squeeze', 'gauge_total_charge'):
-        setattr(_ComplexArray, name, _outofplace(name))
-    # public as np_conserved.ComplexArray: pickle finds the class there (this module's `ComplexArray` is the placeholder)
-    _ComplexArray.__name__ = _ComplexArray.__qualname__ = 'ComplexArray'
-    _ComplexArray.__module__ = npc.__name__
-    return _ComplexArray
-
-
-def complex_product(npc, a, b, prod):
-    """the bilinear product ``prod`` (tensordot, outer) with at least one ComplexArray operand, from the real products
-    of the parts"""
-    CA = npc.ComplexArray
-    a_re, a_im = (a.re, a.im) if isinstance(a, CA) else (a, None)
-    b_re, b_im = (b.re, b.im) if isinstance(b, CA) else (b, None)
-    re = prod(a_re, b_re)
-    if a_im is not None and b_im is not None:
-        re = re - prod(a_im, b_im)
-    im = None
-    if b_im is not None:
-        im = prod(a_re, b_im)
-    if a_im is not None:
-        t = prod(a_im, b_re)
-        im = t if im is None else im + t
-    if not isinstance(re, npc.Array):          # full contraction: scalars
-        return complex(re, im)
-    return CA(re, im)

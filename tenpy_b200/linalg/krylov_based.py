@@ -30,7 +30,7 @@ def _pack(v, lay=None):
     real dot product of the packed planes, and the update, the normalisation and the result assembly have real
     coefficients.  Returns the ComplexArray whose parts are views of the two halves, with the buffer as ``_kbuf``, or
     ``None`` if the table of `v` differs from `lay`."""
-    union, re, im = npc._complex_planes(v)
+    union, (re, im) = npc._planes(v)
     if lay is None:
         lay = union
     elif not (union is lay or union.same_blocks(lay)):
@@ -39,9 +39,7 @@ def _pack(v, lay=None):
     buf = backend.empty(2 * n)
     buf[:n].copy_(re)
     buf[n:].copy_(im)
-    parts = [npc.Array(v.legs, np.float64, v.qtotal, v.get_leg_labels())._set_blocks(lay, half)
-             for half in (buf[:n], buf[n:])]
-    out = npc.ComplexArray(*parts)
+    out = npc._from_planes(v.legs, v.qtotal, lay, (buf[:n], buf[n:]), v.get_leg_labels())
     out._kbuf = buf
     return out
 
@@ -90,14 +88,14 @@ class KrylovBased:
         vf = self._result_krylov
         assert N == len(vf) > 1
         psif = self.psi0 * vf[0]
-        if not isinstance(psif, npc.ComplexArray) and any(isinstance(c, npc.ComplexArray) for c in self._cache):
+        if np.dtype(psif.dtype).kind != 'c' and any(np.dtype(c.dtype).kind == 'c' for c in self._cache):
             psif = psif.astype(np.complex128)        # a real start vector, a complex operator
         len_cache = len(self._cache)
         for k in range(1, min(len_cache + 1, N)):
             psif.iadd_prefactor_other(vf[N - k], self._cache[-k])
         self._cache = []
         self._rebuild_krylov_for_result_full(psif, N - len_cache - 1)
-        if getattr(self, 'device_scalars', False) and isinstance(psif, npc.ComplexArray):
+        if getattr(self, 'device_scalars', False) and np.dtype(psif.dtype).kind == 'c':
             psif = _pack(psif)
         if getattr(self, 'device_scalars', False) and _flat(psif)[0]:
             # normalisation without a host round trip (same arithmetic: |psi|^2 by the dot kernel, x *= 1 / sqrt(.)); the
@@ -162,7 +160,7 @@ class LanczosGroundState(KrylovBased):
         vectors do not share one block layout (caller falls back to the host-scalar loop)."""
         h = self._h_krylov
         lib = backend.get_lib()
-        cplx = isinstance(self.psi0, npc.ComplexArray)
+        cplx = np.dtype(self.psi0.dtype).kind == 'c'
         if cplx:
             self.psi0 = _pack(self.psi0)          # normalised in place below, like a real start vector
         w = self.psi0
@@ -187,9 +185,9 @@ class LanczosGroundState(KrylovBased):
                 w = self.H.matvec(w)
                 v1 = self._cache[-1]
                 if cplx:
-                    w = _pack(w if isinstance(w, npc.ComplexArray) else w.astype(np.complex128), lay)
-                elif isinstance(w, npc.ComplexArray) or not (w._layout is v1._layout or
-                                                             w._layout.same_blocks(v1._layout)):
+                    w = _pack(w if np.dtype(w.dtype).kind == 'c' else w.astype(np.complex128), lay)
+                elif np.dtype(w.dtype).kind == 'c' or not (w._layout is v1._layout or
+                                                           w._layout.same_blocks(v1._layout)):
                     w = None                                  # (a real start vector, a complex operator: host loop)
                 if w is None:
                     if self._psi0_norm is None:
@@ -254,7 +252,7 @@ class LanczosGroundState(KrylovBased):
                 self.H.deferred_check()                                # tests the operator postponed to its first read-back
             h[k, k] = alpha
             self._calc_result_krylov(k)
-            fused = (not self.reortho) and not isinstance(w, npc.ComplexArray) and \
+            fused = (not self.reortho) and np.dtype(w.dtype).kind != 'c' and \
                 w._layout.same_blocks(self._cache[-1]._layout) and \
                 (k == 0 or w._layout.same_blocks(self._cache[-2]._layout))
             if fused:

@@ -89,23 +89,6 @@ def _allowed_qindices(legs, qtotal, chinfo):
     return qd
 
 
-class _WriteThroughBlock(np.ndarray):
-    """host copy of one stored block; assignments are copied to the device buffer (see :meth:`Array.get_block`)"""
-    _target = None
-
-    def __setitem__(self, key, value):
-        if np.iscomplexobj(value):
-            raise TypeError('a block of a real Array can not hold complex values: assign to the blocks of a '
-                            'ComplexArray (.re / .im)')
-        np.ndarray.__setitem__(self, key, value)
-        if self._target is not None:
-            buf, o, s = self._target
-            buf[o:o + s].copy_(backend.to_device(np.ascontiguousarray(np.asarray(self), dtype=np.float64).reshape(-1)))
-
-    def __array_finalize__(self, obj):
-        self._target = None           # views / results of arithmetic are plain host data
-
-
 class Array:
     r"""A block-sparse tensor with abelian charge conservation, stored in packed HBM (reference npc:154).
 
@@ -410,7 +393,7 @@ class Array:
         i = int(match[0])
         o, s = int(lay.offsets[i]), int(lay.sizes[i])
         host = backend.to_host(self._buf[o:o + s]).reshape(lay.shapes[i]).view(_WriteThroughBlock)
-        host._target = (self._buf, o, s)
+        host._targets = ((self._buf, o, s),)
         return host
 
     # ------------------------------------------------------------------ labels
@@ -1205,7 +1188,7 @@ def tensordot(a, b, axes=2, _out=None, _oz_slices=None):
     size without alignment padding, written instead of a fresh allocation (lets a caller place the result inside a
     larger packed buffer)."""
     if isinstance(a, ComplexArray) or isinstance(b, ComplexArray):
-        return _sf.complex_product(_sys.modules[__name__], a, b, lambda x, y: tensordot(x, y, axes))
+        return complex_product(a, b, lambda x, y: tensordot(x, y, axes))
     a, b, n = _prepare_contraction(a, b, axes)
     cut_a = a.rank - n
     if cut_a == 0 and b.rank == n:
@@ -1343,7 +1326,7 @@ def _labels_unique(labels):
 def outer(a, b):
     """Outer product (reference npc:3575), via a contraction over zero legs."""
     if isinstance(a, ComplexArray) or isinstance(b, ComplexArray):
-        return _sf.complex_product(_sys.modules[__name__], a, b, outer)
+        return complex_product(a, b, outer)
     a2, b2, n = _prepare_contraction(a, b, 0)
     res_legs = a.legs + b.legs
     labels = a._labels + b._labels
@@ -1498,7 +1481,7 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
     A :class:`ComplexArray` `a` is decomposed by the complex block-Jacobi kernel (``b200_block_svd_z``) with the same
     charges, legs and options; `U` and `VH` are then ComplexArrays and `S` is real.  `guess` is not supported for
     complex input (NotImplementedError)."""
-    if guess is not None and isinstance(a, ComplexArray):
+    if guess is not None and a.dtype.kind == 'c':
         raise NotImplementedError('svd: `guess` (warm start) is only implemented for real Arrays')
     if deflation_tol is None:
         deflation_tol = SVD_DEFAULTS['deflation_tol']        # module-wide default (None: rounding level only)
@@ -1559,11 +1542,7 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
         raise ValueError('The entries of `qtotal_LR` have to add up to ``a.qtotal``!')
     qtotal_L = chinfo.make_valid(qtotal_L)
     qtotal_R = chinfo.make_valid(qtotal_R)
-    cplx = isinstance(a, ComplexArray)
-    if cplx:
-        lay, bufA_re, bufA_im = _complex_planes(a)
-    else:
-        lay = a._layout
+    lay, A = _planes(a)
     if lay.nblocks == 0:
         raise RuntimeError('SVD found no singular values')
     m = lay.shapes[:, 0]
@@ -1576,35 +1555,26 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
     new_leg_R = LegCharge.from_qind(chinfo, s_off, new_charges, inner_qconj)
     new_leg_L = new_leg_R.conj()
     qi_C = np.arange(lay.nblocks, dtype=np.int64)
-    U = Array([a.legs[0], new_leg_L], np.float64, qtotal_L)
-    VH = Array([new_leg_R, a.legs[1]], np.float64, qtotal_R)
-    lay_U, perm_U = BlockLayout.from_legs(U.legs, np.stack([qi_L, qi_C], axis=1))
-    lay_V, perm_V = BlockLayout.from_legs(VH.legs, np.stack([qi_C, qi_R], axis=1))
+    U_legs, VH_legs = [a.legs[0], new_leg_L], [new_leg_R, a.legs[1]]
+    lay_U, perm_U = BlockLayout.from_legs(U_legs, np.stack([qi_L, qi_C], axis=1))
+    lay_V, perm_V = BlockLayout.from_legs(VH_legs, np.stack([qi_C, qi_R], axis=1))
     u_off = np.empty(lay.nblocks, dtype=np.int64)
     v_off = np.empty(lay.nblocks, dtype=np.int64)
     u_off[perm_U] = lay_U.offsets
     v_off[perm_V] = lay_V.offsets
     lib = backend.get_lib()
-    bufU = backend.zeros(lay_U.size)
-    bufV = backend.zeros(lay_V.size)
+    bufU = tuple(backend.zeros(lay_U.size) for _ in A)        # one output plane per input plane
+    bufV = tuple(backend.zeros(lay_V.size) for _ in A)
     bufS = backend.empty(int(s_off[-1]))
-    if cplx:
-        bufU_im = backend.zeros(lay_U.size)
-        bufV_im = backend.zeros(lay_V.size)
-        info, nact, transp = lib.block_svd_z(m, n, lay.offsets, u_off, s_off[:-1], v_off, bufA_re, bufA_im, bufU, bufU_im,
-                                             bufS, bufV, bufV_im)
-    else:
-        info, nact, transp = lib.block_svd(m, n, lay.offsets, u_off, s_off[:-1], v_off, a._buf, bufU, bufS, bufV)
+    block_svd = lib.block_svd if len(A) == 1 else lib.block_svd_z
+    info, nact, transp = block_svd(m, n, lay.offsets, u_off, s_off[:-1], v_off, *A, *bufU, bufS, *bufV)
     svd_stats['calls'] += 1
     svd_stats['jacobi_sweeps'].append(int(np.max(info)))
     if np.any(nact < k):
         # numerically rank-deficient blocks: the kernel left the vectors of the negligible directions on one side zero;
         # complete them to an orthonormal basis (LAPACK returns a complete basis, reference npc:4950).  Real blocks: GEMM-only
         # Newton-Schulz, which can fail on an ill-conditioned start; complex blocks: the complex QR kernel, which cannot
-        if cplx:
-            fill, fill_U, fill_V = _fill_null_vectors_z, (bufU, bufU_im), (bufV, bufV_im)
-        else:
-            fill, fill_U, fill_V = _fill_null_vectors, bufU, bufV
+        fill = _fill_null_vectors if len(A) == 1 else _fill_null_vectors_z
         S_h = backend.to_host(bufS).copy()
         try:
             for i in np.nonzero(nact < k)[0]:
@@ -1612,8 +1582,8 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
                 k_fill = int(k[i]) if n_keep is None else min(int(k[i]), max(int(n_keep), int(nact[i])))
                 n_fill = k_fill - int(nact[i])
                 if n_fill > 0:
-                    fill(lib, int(m[i]), int(n[i]), int(k[i]), int(nact[i]), n_fill, bool(transp[i]), fill_U, int(u_off[i]),
-                         fill_V, int(v_off[i]))
+                    fill(lib, int(m[i]), int(n[i]), int(k[i]), int(nact[i]), n_fill, bool(transp[i]), bufU, int(u_off[i]),
+                         bufV, int(v_off[i]))
                 # singular values of the negligible directions: tiny but positive for the completed vectors (so that a
                 # truncation prefers them), exactly zero for the ones left without a vector
                 lo, hi = int(s_off[i]) + int(nact[i]), int(s_off[i]) + int(k[i])
@@ -1624,9 +1594,9 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
             svd_stats['completion_fallbacks'] = svd_stats.get('completion_fallbacks', 0) + 1
             old = lib.svd_set_deflation(False)
             try:
-                bufU.zero_()
-                bufV.zero_()
-                info, nact, transp = lib.block_svd(m, n, lay.offsets, u_off, s_off[:-1], v_off, a._buf, bufU, bufS, bufV)
+                for buf in bufU + bufV:
+                    buf.zero_()
+                info, nact, transp = block_svd(m, n, lay.offsets, u_off, s_off[:-1], v_off, *A, *bufU, bufS, *bufV)
             finally:
                 lib.svd_set_deflation(old)
         else:
@@ -1639,12 +1609,8 @@ def svd(a, full_matrices=False, compute_uv=True, cutoff=None, qtotal_LR=[None, N
         if cutoff is not None:
             S = S[S > cutoff]
         return S
-    U._set_blocks(lay_U, bufU)
-    VH._set_blocks(lay_V, bufV)
-    if cplx:
-        U_im = Array(U.legs, np.float64, U.qtotal)._set_blocks(lay_U, bufU_im)
-        VH_im = Array(VH.legs, np.float64, VH.qtotal)._set_blocks(lay_V, bufV_im)
-        U, VH = ComplexArray(U, U_im), ComplexArray(VH, VH_im)
+    U = _from_planes(U_legs, qtotal_L, lay_U, bufU)
+    VH = _from_planes(VH_legs, qtotal_R, lay_V, bufV)
     if cutoff is not None:
         keep = S > cutoff
         if not np.any(keep):
@@ -1759,8 +1725,10 @@ def _null_space_completion(lib, V, r, p, kf):
     raise _CompletionFailed('Newton-Schulz did not converge')
 
 
-def _fill_null_vectors(lib, m, n, k, r, kf, transposed, bufU, u_off, bufV, v_off):
-    """fill `kf` of the zero vectors left by the deflating SVD kernel for block (m x n), see b200_block_svd_f64"""
+def _fill_null_vectors(lib, m, n, k, r, kf, transposed, planesU, u_off, planesV, v_off):
+    """fill `kf` of the zero vectors left by the deflating SVD kernel for block (m x n), see b200_block_svd_f64
+    (`planesU`, `planesV` = the one plane of U and VT)"""
+    (bufU,), (bufV,) = planesU, planesV
     if not transposed:           # rows r..k-1 of VT (k x n) are missing; the first r rows are orthonormal
         V = bufV[v_off:v_off + max(r, 1) * n]
         X = _null_space_completion(lib, V, r, n, kf)
@@ -1811,23 +1779,6 @@ def _fill_null_vectors_z(lib, m, n, k, r, kf, transposed, bufU, u_off, bufV, v_o
             _strided_copy(lib, Q[part], r, bufU[part], u_off + r, [p, kf], [c, 1], [k, 1])
         else:                       # rows r.. of VT <- columns r.. of Q
             _strided_copy(lib, Q[part], r, bufV[part], v_off + r * n, [kf, p], [1, c], [p, 1])
-
-
-def _complex_planes(a):
-    """``(layout, buf_re, buf_im)``: the two parts of the ComplexArray `a` on ONE block table.  Each part drops its own
-    zero blocks, so their tables can differ; a block missing in one part is a zero block there."""
-    lr, li = a.re._layout, a.im._layout
-    if lr.same_blocks(li):
-        return lr, a.re._buf, a.im._buf
-    union, seg_re, seg_im = _union_layout(a.legs, lr, li)
-    lib = backend.get_lib()
-    bufs = []
-    for seg, part in ((seg_re, a.re), (seg_im, a.im)):
-        buf = backend.zeros(union.size)
-        if len(seg):
-            lib.axpy_segments(len(seg), backend.to_device(seg), int(seg[:, 2].max()), 1.0, part._buf, buf)
-        bufs.append(buf)
-    return union, bufs[0], bufs[1]
 
 
 qr_stats = {'calls': 0, 'columns': 0, 'replaced': 0}   # diagnostics of the Gram-Schmidt QR
@@ -1941,11 +1892,7 @@ def qr(a, mode='reduced', inner_labels=[None, None], cutoff=None, pos_diag_R=Fal
     label_Q, label_R = inner_labels
     piped_axes, a = a.as_completely_blocked()
     chinfo = a.chinfo
-    cplx = isinstance(a, ComplexArray)
-    if cplx:
-        lay, bufA_re, bufA_im = _complex_planes(a)
-    else:
-        lay = a._layout
+    lay, A = _planes(a)
     a_leg0 = a.legs[0]
     m, n = lay.shapes[:, 0], lay.shapes[:, 1]
     k = np.minimum(m, n)
@@ -1965,42 +1912,37 @@ def qr(a, mode='reduced', inner_labels=[None, None], cutoff=None, pos_diag_R=Fal
         charges_in = chinfo.make_valid(-charges_in)
         qc = inner_qconj
     inner_leg = LegCharge.from_qind(chinfo, inner_leg.slices, charges_in, qc)
-    Q = Array([a_leg0, inner_leg.conj()], np.float64, qtotal_Q)
-    R = Array([inner_leg, a.legs[1]], np.float64, chinfo.make_valid(a.qtotal - Q.qtotal))
+    Q_legs, R_legs = [a_leg0, inner_leg.conj()], [inner_leg, a.legs[1]]
+    qtotal_Q = chinfo.make_valid(qtotal_Q)
+    lay_Q = lay_R = None                      # no blocks
+    bufQ = bufR = (None,) * len(A)
     if lay.nblocks:
         qi_C = map_qind[lay.qdata[:, 0]].astype(np.int64)
-        lay_Q, perm_Q = BlockLayout.from_legs(Q.legs, np.stack([lay.qdata[:, 0], qi_C], axis=1))
-        lay_R, perm_R = BlockLayout.from_legs(R.legs, np.stack([qi_C, lay.qdata[:, 1]], axis=1))
+        lay_Q, perm_Q = BlockLayout.from_legs(Q_legs, np.stack([lay.qdata[:, 0], qi_C], axis=1))
+        lay_R, perm_R = BlockLayout.from_legs(R_legs, np.stack([qi_C, lay.qdata[:, 1]], axis=1))
         q_off = np.empty(lay.nblocks, dtype=np.int64)
         r_off = np.empty(lay.nblocks, dtype=np.int64)
         q_off[perm_Q] = lay_Q.offsets
         r_off[perm_R] = lay_R.offsets
-        bufQ = backend.zeros(lay_Q.size)
-        bufR = backend.zeros(lay_R.size)
+        bufQ = tuple(backend.zeros(lay_Q.size) for _ in A)        # one output plane per input plane
+        bufR = tuple(backend.zeros(lay_R.size) for _ in A)
         lib = backend.get_lib()
-        if cplx:         # complex: the Householder kernel for every block size
-            Q_im, R_im = Array(Q.legs, np.float64, Q.qtotal), Array(R.legs, np.float64, R.qtotal)
-            bufQ_im = backend.zeros(lay_Q.size)
-            bufR_im = backend.zeros(lay_R.size)
-            lib.block_qr_z(m, n, lay.offsets, q_off, r_off, bufA_re, bufA_im, bufQ, bufQ_im, bufR, bufR_im)
-            Q_im._set_blocks(lay_Q, bufQ_im)
-            R_im._set_blocks(lay_R, bufR_im)
+        # the Householder kernel in one launch: complex blocks of every size, real blocks up to QR_HOUSEHOLDER_MAX; larger
+        # real blocks: Gram-Schmidt
+        if len(A) == 1:
+            block_qr, small = lib.block_qr, np.maximum(m, n) <= QR_HOUSEHOLDER_MAX
         else:
-            small = np.maximum(m, n) <= QR_HOUSEHOLDER_MAX
-            if np.any(small):
-                lib.block_qr(m[small], n[small], lay.offsets[small], q_off[small], r_off[small], a._buf, bufQ, bufR)
-            for b in np.nonzero(~small)[0]:
-                mb, nb, kb = int(m[b]), int(n[b]), int(k[b])
-                ao = int(lay.offsets[b])
-                _block_qr_cgs2(lib, mb, nb, a._buf[ao:ao + mb * nb], bufQ[int(q_off[b]):int(q_off[b]) + mb * kb],
-                               bufR[int(r_off[b]):int(r_off[b]) + kb * nb])
-        Q._set_blocks(lay_Q, bufQ)
-        R._set_blocks(lay_R, bufR)
+            block_qr, small = lib.block_qr_z, np.ones(lay.nblocks, dtype=np.bool_)
+        if np.any(small):
+            block_qr(m[small], n[small], lay.offsets[small], q_off[small], r_off[small], *A, *bufQ, *bufR)
+        for b in np.nonzero(~small)[0]:
+            mb, nb, kb = int(m[b]), int(n[b]), int(k[b])
+            ao = int(lay.offsets[b])
+            _block_qr_cgs2(lib, mb, nb, A[0][ao:ao + mb * nb], bufQ[0][int(q_off[b]):int(q_off[b]) + mb * kb],
+                           bufR[0][int(r_off[b]):int(r_off[b]) + kb * nb])
         qr_stats['calls'] += 1
-    elif cplx:
-        Q_im, R_im = Array(Q.legs, np.float64, Q.qtotal), Array(R.legs, np.float64, R.qtotal)
-    if cplx:
-        Q, R = ComplexArray(Q, Q_im), ComplexArray(R, R_im)
+    Q = _from_planes(Q_legs, qtotal_Q, lay_Q, bufQ)
+    R = _from_planes(R_legs, chinfo.make_valid(a.qtotal - qtotal_Q), lay_R, bufR)
     if 0 in piped_axes:
         Q = Q.split_legs(0)
     if 1 in piped_axes:
@@ -2046,13 +1988,12 @@ def eigh(a, UPLO='L', sort=None):
     A :class:`ComplexArray` `a` must be Hermitian to ``|a - a^H|_F <= 1e-8 |a|_F`` (else NotImplementedError: only
     Hermitian eigenproblems are provided); it goes through the complex block-Jacobi kernel (``b200_block_eigh_z``), `W`
     is real and `V` a ComplexArray."""
-    cplx = isinstance(a, ComplexArray)
     if a.rank != 2 or a.shape[0] != a.shape[1]:
         raise ValueError('expect a square matrix!')
     a.legs[0].test_contractible(a.legs[1])
     if np.any(a.qtotal != a.chinfo.make_valid()):
         raise ValueError('Non-trivial qtotal -> Nilpotent. Not diagonizable!?')
-    if cplx:
+    if a.dtype.kind == 'c':
         defect2, norm2 = _hermitian_defect(a)
         if not defect2 <= 1e-16 * norm2:
             raise NotImplementedError('eigh: the ComplexArray is not complex Hermitian (|A - A^H|_F = {0:.3g} |A|_F); '
@@ -2061,10 +2002,7 @@ def eigh(a, UPLO='L', sort=None):
     a_label0 = a._labels[0]
     piped_axes, a = a.as_completely_blocked()
     leg = a.legs[0]
-    if cplx:
-        lay, bufA, bufA_im = _complex_planes(a)
-    else:
-        lay, bufA = a._layout, a._buf
+    lay, A = _planes(a)
     if np.any(lay.qdata[:, 0] != lay.qdata[:, 1]):
         raise ValueError('off-diagonal blocks in a completely blocked matrix with zero charge?')
     resw = np.zeros(a.shape[0], dtype=np.float64)
@@ -2072,9 +2010,9 @@ def eigh(a, UPLO='L', sort=None):
     nbk = leg.block_number
     sizes = leg.get_block_sizes().astype(np.int64)
     leg2 = a.legs[1].to_LegCharge() if isinstance(a.legs[1], LegPipe) else a.legs[1]
-    V = Array([leg, leg2], np.float64, None)
+    V_legs = [leg, leg2]
     qd = np.arange(nbk, dtype=np.int64)
-    lay_V = BlockLayout.from_legs(V.legs, np.stack([qd, qd], axis=1), presorted=True)[0]
+    lay_V = BlockLayout.from_legs(V_legs, np.stack([qd, qd], axis=1), presorted=True)[0]
     stored = lay.qdata[:, 0]
     missing = np.setdiff1d(qd, stored)
     if len(missing):
@@ -2086,18 +2024,14 @@ def eigh(a, UPLO='L', sort=None):
         bufV = backend.to_device(host)
     else:
         bufV = backend.zeros(lay_V.size)
-    planes = [bufV]
-    if cplx:
-        planes.append(backend.zeros(lay_V.size))
+    planes = (bufV,) + tuple(backend.zeros(lay_V.size) for _ in A[1:])       # one output plane per input plane
     if lay.nblocks:
         lib = backend.get_lib()
         nn = sizes[stored]
         w_off = np.concatenate(([0], np.cumsum(nn)))
         bufW = backend.empty(int(w_off[-1]))
-        if cplx:
-            lib.block_eigh_z(nn, lay.offsets, w_off[:-1], lay_V.offsets[stored], bufA, bufA_im, bufW, bufV, planes[1])
-        else:
-            lib.block_eigh(nn, lay.offsets, w_off[:-1], lay_V.offsets[stored], bufA, bufW, bufV)
+        block_eigh = lib.block_eigh if len(A) == 1 else lib.block_eigh_z
+        block_eigh(nn, lay.offsets, w_off[:-1], lay_V.offsets[stored], *A, bufW, *planes)
         w = backend.to_host(bufW)
         recs, pool, at = [], [], 0
         for j, qi in enumerate(stored):
@@ -2122,11 +2056,7 @@ def eigh(a, UPLO='L', sort=None):
             for buf in planes:
                 src = buf.clone()
                 lib.take_blocks(rec, rec_dev, pool_dev, src, buf)
-    V._set_blocks(lay_V, bufV)
-    if cplx:
-        V_im = Array(V.legs, np.float64, None)
-        V_im._set_blocks(lay_V, planes[1])
-        V = ComplexArray(V, V_im)
+    V = _from_planes(V_legs, None, lay_V, planes)
     if len(piped_axes) > 0:
         V = V.split_legs(0)
     V.iset_leg_labels([a_label0, 'eig'] if a_label0 != 'eig' else [None, 'eig'])
@@ -2146,9 +2076,8 @@ def concatenate_qdata(*a):  # pragma: no cover - placeholder for API completenes
 
 
 # ---- the rest of the reference's surface (cold paths: model / MPO / site construction, indexing, complex tensors) ----------
-import sys as _sys
-
 from . import _surface as _sf
+from ._complex import ComplexArray, _WriteThroughBlock, _planes, _from_planes, complex_product
 from .charges import DipolarChargeInfo
 from ._surface import (QCUTOFF, grid_outer, grid_concat, detect_grid_outer_legcharge, detect_legcharge, eig, eigvals,
                        speigs, expm, lq, polar, orthogonal_columns)
@@ -2170,7 +2099,6 @@ Array.drop_charge = _sf.array_drop_charge
 Array.change_charge = _sf.array_change_charge
 Array.shift_charges = _sf.array_shift_charges
 Array.shift_charges_horizontal = _sf.array_shift_charges_horizontal
-ComplexArray = _sf._finish_complex(_sys.modules[__name__])
 
 __all__ += ['DipolarChargeInfo', 'QCUTOFF', 'ComplexArray', 'grid_outer', 'grid_concat', 'detect_grid_outer_legcharge',
             'detect_legcharge', 'eig', 'eigvals', 'speigs', 'expm', 'lq', 'polar', 'orthogonal_columns']

@@ -42,13 +42,8 @@ def run_case(Engine=None):
 def main(mode):
     from run_reference_drivers import setup
     dropin = setup(mode)
-    if mode == 'fake':       # the numpy test double with the complex decompositions and the complex eigh
-        from tenpy_b200 import backend
-        from fake_device_eigh_z import FakeEighZDeviceLib
-        lib = backend.use_library(FakeEighZDeviceLib())
-    else:
-        from tenpy_b200 import backend
-        lib = backend.get_lib()
+    from tenpy_b200 import backend
+    lib = backend.get_lib()
     out = {'reference_engine': run_case(), 'fast_engine': run_case(dropin.fast_two_site_engine())}
     if mode == 'fake':
         out['eigh_z_calls'] = lib.calls.get('block_eigh_z', 0)

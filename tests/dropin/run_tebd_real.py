@@ -84,10 +84,6 @@ def run_cases():
 def main(mode):
     from run_reference_drivers import setup
     setup(mode)
-    if mode == 'fake':       # the numpy test double with the complex decompositions (tests/fake_device_complex.py)
-        from tenpy_b200 import backend
-        from fake_device_complex import FakeComplexDeviceLib
-        backend.use_library(FakeComplexDeviceLib())
     print(json.dumps(run_cases()))
 
 

@@ -88,6 +88,21 @@ def ozaki_product(a, b):
     return C
 
 
+def _get_block(planes, off, shape):
+    """the block at `off` of the device planes (one: real, two: real and imaginary) as a host array"""
+    size = int(np.prod(shape))
+    blk = planes[0].numpy()[off:off + size]
+    if len(planes) == 2:
+        blk = blk + 1.j * planes[1].numpy()[off:off + size]
+    return blk.reshape(shape)
+
+
+def _put_block(planes, off, blk):
+    """write the host block `blk` at `off` of the device planes (one: real, two: real and imaginary)"""
+    for plane, part in zip(planes, (np.real, np.imag)):
+        plane.numpy()[off:off + blk.size] = part(blk).reshape(-1)
+
+
 def fro_norm(blk):
     """|blk|_F without over- or underflow (the kernels scale every block by a power of two first)"""
     amax = np.max(np.abs(blk), initial=0.)
@@ -249,36 +264,59 @@ class FakeDeviceLib:
         return int(old)
 
     def block_svd(self, m, n, a_off, u_off, s_off, vt_off, A, U, S, VT):
-        """numpy SVD; emulates the kernel's deflation contract (zero VT rows for negligible directions)"""
         self._count('block_svd')
-        a, u, s, vt = A.numpy(), U.numpy(), S.numpy(), VT.numpy()
+        return self._svd(m, n, a_off, u_off, s_off, vt_off, (A,), (U,), S, (VT,))
+
+    def block_svd_z(self, m, n, a_off, u_off, s_off, vt_off, A_re, A_im, U_re, U_im, S, VT_re, VT_im):
+        self._count('block_svd_z')
+        return self._svd(m, n, a_off, u_off, s_off, vt_off, (A_re, A_im), (U_re, U_im), S, (VT_re, VT_im))
+
+    def _svd(self, m, n, a_off, u_off, s_off, vt_off, A, U, S, VT):
+        """numpy SVD; emulates the kernel's deflation contract: the vectors of the negligible directions are left zero on
+        one side.  Real blocks: always rows of VT.  Complex blocks: a block with m >= n is orthogonalised on its columns
+        (``transposed`` = 1, zero columns of U), other blocks on their rows (zero rows of VT), so both completion paths
+        of ``npc.svd`` run on the CPU."""
+        s = S.numpy()
         nact = np.zeros(len(m), dtype=np.int32)
+        transp = np.zeros(len(m), dtype=np.int32)
         for i in range(len(m)):
             mi, ni = int(m[i]), int(n[i])
             k = min(mi, ni)
-            blk = a[a_off[i]:a_off[i] + mi * ni].reshape(mi, ni)
+            blk = _get_block(A, a_off[i], (mi, ni))
             uu, ss, vv = np.linalg.svd(blk, full_matrices=False)
             defl = max(16 * 2.220446049250313e-16 * np.sqrt(max(mi, ni)), self.deflation_tol) * fro_norm(blk) \
                 if self.deflation else -1.
             r = int(np.sum(ss > defl))
-            vv = vv.copy()
-            vv[r:] = 0.
+            uu, vv = uu.copy(), vv.copy()
+            if len(A) == 2 and mi >= ni:
+                transp[i] = 1
+                uu[:, r:] = 0.
+            else:
+                vv[r:] = 0.
             nact[i] = r
-            u[u_off[i]:u_off[i] + mi * k] = uu.reshape(-1)
+            _put_block(U, u_off[i], uu)
             s[s_off[i]:s_off[i] + k] = ss
-            vt[vt_off[i]:vt_off[i] + k * ni] = vv.reshape(-1)
-        return np.ones(len(m), dtype=np.int32), nact, np.zeros(len(m), dtype=np.int32)
+            _put_block(VT, vt_off[i], vv)
+        return np.ones(len(m), dtype=np.int32), nact, transp
 
     def block_qr(self, m, n, a_off, q_off, r_off, A, Q, R):
         self._count('block_qr')
-        a, q, r = A.numpy(), Q.numpy(), R.numpy()
+        self._qr(m, n, a_off, q_off, r_off, (A,), (Q,), (R,))
+
+    def block_qr_z(self, m, n, a_off, q_off, r_off, A_re, A_im, Q_re, Q_im, R_re, R_im):
+        self._count('block_qr_z')
+        self._qr(m, n, a_off, q_off, r_off, (A_re, A_im), (Q_re, Q_im), (R_re, R_im))
+
+    def _qr(self, m, n, a_off, q_off, r_off, A, Q, R):
+        """numpy QR, R with a real non-negative diagonal: the phase (for a real block the sign) of each diagonal entry
+        moves into the column of Q"""
         for i in range(len(m)):
-            mi, ni = int(m[i]), int(n[i])
-            k = min(mi, ni)
-            qq, rr = np.linalg.qr(a[a_off[i]:a_off[i] + mi * ni].reshape(mi, ni))
-            sgn = np.where(np.diag(rr) < 0., -1., 1.)
-            q[q_off[i]:q_off[i] + mi * k] = (qq * sgn[None, :]).reshape(-1)
-            r[r_off[i]:r_off[i] + k * ni] = (rr * sgn[:, None]).reshape(-1)
+            qq, rr = np.linalg.qr(_get_block(A, a_off[i], (int(m[i]), int(n[i]))))
+            d = np.diag(rr)
+            ad = np.abs(d)
+            ph = np.where(ad > 0., d / np.where(ad > 0., ad, 1.), 1.)
+            _put_block(Q, q_off[i], qq * ph[None, :])
+            _put_block(R, r_off[i], rr * ph.conj()[:, None])
 
     def col_sqnorms(self, rows, cols, ld, X, OUT):
         self._count('col_sqnorms')
@@ -297,10 +335,20 @@ class FakeDeviceLib:
 
     def block_eigh(self, n, a_off, w_off, v_off, A, W, V):
         self._count('block_eigh')
-        a, w, v = A.numpy(), W.numpy(), V.numpy()
+        return self._eigh(n, a_off, w_off, v_off, (A,), W, (V,))
+
+    def block_eigh_z(self, n, a_off, w_off, v_off, A_re, A_im, W, V_re, V_im):
+        self._count('block_eigh_z')
+        return self._eigh(n, a_off, w_off, v_off, (A_re, A_im), W, (V_re, V_im))
+
+    def _eigh(self, n, a_off, w_off, v_off, A, W, V):
+        """numpy eigh, W ascending, the eigenvectors in the columns of V; like the kernel, a complex block is taken as
+        (A + A^H) / 2"""
+        w = W.numpy()
         for i in range(len(n)):
             ni = int(n[i])
-            ww, vv = np.linalg.eigh(a[a_off[i]:a_off[i] + ni * ni].reshape(ni, ni))
+            blk = _get_block(A, a_off[i], (ni, ni))
+            ww, vv = np.linalg.eigh(blk if len(A) == 1 else 0.5 * (blk + blk.conj().T))
             w[w_off[i]:w_off[i] + ni] = ww
-            v[v_off[i]:v_off[i] + ni * ni] = vv.reshape(-1)
+            _put_block(V, v_off[i], vv)
         return np.ones(len(n), dtype=np.int32)

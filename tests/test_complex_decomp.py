@@ -1,6 +1,6 @@
 """Complex decompositions: the kernels b200_block_svd_z / b200_block_qr_z against numpy on complex128 (GPU), and
 npc.svd / npc.qr / npc.inner of charge-conserving ComplexArrays against dense numpy (GPU and the CPU test double of
-tests/fake_device_complex.py).
+tests/fake_device.py).
 
 Kernel checks follow tests/test_gpu_kernel_edges.py: output buffers are NaN-filled, blocks are laid out with gaps, and every
 element outside the blocks must stay untouched.  Bounds (eps = 2^-52, k = min(m, n), p = max(m, n)):
@@ -226,12 +226,8 @@ KINDS = ['same', 'differ', 'rankdef']
 
 
 @pytest.fixture
-def fake_device_z():
-    """the numpy test double of the device library with the complex decompositions (tests/fake_device_complex.py)"""
-    import fake_device_complex
-    lib, restore = fake_device_complex.install()
-    yield lib
-    restore()
+def fake_device_z(fake_device):
+    return fake_device
 
 
 def _npc_svd_case(kind):

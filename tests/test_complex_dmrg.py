@@ -1,5 +1,5 @@
 """Ground-state DMRG of complex Hamiltonians on the engine's own driver (two-site engine, `models.SpinChain` with a
-Dzyaloshinskii-Moriya term `D`), on the CPU test double (tests/fake_device_eigh_z.py) at small L and on the GPU larger.
+Dzyaloshinskii-Moriya term `D`), on the CPU test double (tests/fake_device.py) at small L and on the GPU larger.
 
 * Gauge test: with ``Jx = Jy = J`` the DM term only twists the XY coupling, ``(J + iD)/2 S+_i S-_{i+1} + h.c.``; on an
   open chain ``prod_j exp(-i j phi Sz_j)`` removes the phase, so the chain is equivalent to the real XXZ chain with
@@ -13,11 +13,8 @@ import pytest
 
 
 @pytest.fixture
-def fake_device_eigh_z():
-    import fake_device_eigh_z
-    lib, restore = fake_device_eigh_z.install()
-    yield lib
-    restore()
+def fake_device_eigh_z(fake_device):
+    return fake_device
 
 
 MIXER_PARAMS = {'amplitude': 1e-5, 'decay': 2., 'disable_after': 6}

@@ -1,6 +1,6 @@
 """Complex Hermitian eigen-decomposition: the kernel b200_block_eigh_z against numpy.linalg.eigh on dense complex
 Hermitian blocks (GPU), and npc.eigh / npc.eigvalsh of charge-conserving ComplexArrays against dense numpy (GPU and the
-CPU test double of tests/fake_device_eigh_z.py).
+CPU test double of tests/fake_device.py).
 
 Kernel bounds, in the units of test_gpu_kernel_edges._check_eigh (p = max(n, 16), eps = 2^-52):
 * eigenvalues |W - W_ref|_max and residual |A V - V W|_max <= 4 p eps |A|_F
@@ -171,12 +171,8 @@ def test_block_eigh_z_scale_equivariance(gpu_lib, big):
 # ---- npc ------------------------------------------------------------------------------------------------------------------
 
 @pytest.fixture
-def fake_device_eigh_z():
-    """the numpy test double with the complex decompositions and the complex eigh (tests/fake_device_eigh_z.py)"""
-    import fake_device_eigh_z
-    lib, restore = fake_device_eigh_z.install()
-    yield lib
-    restore()
+def fake_device_eigh_z(fake_device):
+    return fake_device
 
 
 CHARGES = ['U1', 'Z2', 'U1xZ2']

@@ -1,16 +1,13 @@
 """Lanczos on complex vectors: the ground state of a random complex Hermitian block-sparse operator against dense numpy,
 through the device-scalar route (both planes of a Krylov vector in one buffer, one dot launch per iteration) and through
-the host-scalar loop, on the CPU test double (tests/fake_device_eigh_z.py) and on the GPU."""
+the host-scalar loop, on the CPU test double (tests/fake_device.py) and on the GPU."""
 import numpy as np
 import pytest
 
 
 @pytest.fixture
-def fake_device_eigh_z():
-    import fake_device_eigh_z
-    lib, restore = fake_device_eigh_z.install()
-    yield lib
-    restore()
+def fake_device_eigh_z(fake_device):
+    return fake_device
 
 
 class _Op:

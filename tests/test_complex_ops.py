@@ -1,8 +1,8 @@
-"""Randomised differential test of the complex tensor layer (`ComplexArray`, tenpy_b200/linalg/_surface.py) against dense
+"""Randomised differential test of the complex tensor layer (`ComplexArray`, tenpy_b200/linalg/_complex.py) against dense
 complex128 NumPy, in the manner of tests/test_random_ops.py for the real Arrays: random charge rules (none, U(1),
 U(1)xZ2, Z3), random legs (sorted or not, unbunched, ragged block sizes), random total charges incl. ones that allow no
 block at all, and real and imaginary parts with different block tables.  Runs on the numpy test double with the complex
-decompositions (tests/fake_device_complex.py) and, marked ``gpu``, on the CUDA kernels.
+decompositions (tests/fake_device.py) and, marked ``gpu``, on the CUDA kernels.
 
 Reference rules:
 * data movement, conjugation, sums and scaling by real factors or powers of two round once or not at all: they must
@@ -28,12 +28,8 @@ KINDS = ['both', 'im_subset', 'im_empty', 're_empty', 'im_zero', 're_zero']
 
 
 @pytest.fixture
-def fake_device_z():
-    """the numpy test double of the device library with the complex decompositions (tests/fake_device_complex.py)"""
-    import fake_device_complex
-    lib, restore = fake_device_complex.install()
-    yield lib
-    restore()
+def fake_device_z(fake_device):
+    return fake_device
 
 
 # ---- random complex tensors ---------------------------------------------------------------------------------------------
