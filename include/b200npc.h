@@ -187,7 +187,10 @@ int b200_scale_axis_f64(int64_t n_tasks, const int64_t *task_dev, const int64_t 
  * device scratch of b200_block_qr_worksize bytes.  npc.qr uses it for real blocks of up to 384 rows and columns
  * (np_conserved.QR_HOUSEHOLDER_MAX).
  * Range: every finite block.  Each block is factored as 2^-e A_i, 2^e the power of two of max |a_ij| (exact), and R is
- * scaled back by 2^e: Q is bit for bit that of 2^-e A_i and R exactly 2^e times its R (rounded once where it is subnormal). */
+ * scaled back by 2^e: Q is bit for bit that of 2^-e A_i and R exactly 2^e times its R (rounded once where it is subnormal).
+ * A pivot column of 2^-e A_i whose norm from the diagonal down is below 2^-450 is negligible: it gets no reflector, and
+ * its entries below the diagonal (and the imaginary part of its diagonal entry) are dropped, so that columns many
+ * orders of magnitude below the largest one cannot make Q non-orthogonal or non-finite. */
 int64_t b200_block_qr_worksize(int64_t nblocks, const int64_t *m_host, const int64_t *n_host);
 int b200_block_qr_f64(int64_t nblocks, const int64_t *m_host, const int64_t *n_host, const int64_t *a_off_host,
                       const int64_t *q_off_host, const int64_t *r_off_host, const double *A, double *Q, double *R,

@@ -86,23 +86,32 @@ BQ_HD void col_partial(int tid, int T, const double *A, int m, int n, int j, dou
     partial[tid] = s;
 }
 
+// A pivot column whose squared norm from the diagonal down is below this is negligible: the block is scaled so that
+// max |a_ij| >= 2^-52, and the column is below 2^-450.  Its squares are subnormal or zero, so its norm would be
+// inaccurate (a non-orthogonal reflector) or zero with alpha != 0 (tau and scale infinite).
+constexpr double QR_NEGLIGIBLE_SQNORM = 0x1p-900;
+
 // PHASE 2 (one thread): reflector H = 1 - tau v v^H with v[j] = 1 that maps the pivot column to beta e_j (H^H for a
 // complex block), beta real: beta = -sign(Re alpha) |column from the diagonal down|, tau = (beta - alpha) / beta,
 // scale = 1 / (alpha - beta).  params[0] = Re tau, params[1] = Re scale (v[r] = A[r][j] * scale for r > j),
-// params[2] = beta; a complex block (Ai not NULL) also writes params[3] = Im tau, params[4] = Im scale
+// params[2] = beta; a complex block (Ai not NULL) also writes params[3] = Im tau, params[4] = Im scale.
+// H = 1 (tau = scale = 0, beta = Re alpha) where the column below the diagonal and Im alpha are zero, and where the
+// column is negligible (QR_NEGLIGIBLE_SQNORM): store_reflector then drops its entries below the diagonal and Im alpha,
+// an absolute change below 2^-450 of a block whose largest entry is >= 2^-52.
 BQ_HD void reflector(int T, const double *A, int n, int j, const double *partial, double *params,
                      const double *Ai = nullptr) {
     double sigma = 0.0;
     for (int t = 0; t < T; ++t) sigma += partial[t];
     const double alpha = A[(int64_t)j * n + j], ai = Ai ? Ai[(int64_t)j * n + j] : 0.0;
     if (Ai) params[3] = params[4] = 0.0;
-    if (sigma == 0.0 && ai == 0.0) {                  // H = 1
+    const double nrm2 = Ai ? fma(alpha, alpha, fma(ai, ai, sigma)) : alpha * alpha + sigma;
+    if ((sigma == 0.0 && ai == 0.0) || nrm2 < QR_NEGLIGIBLE_SQNORM) {   // H = 1
         params[0] = 0.0;
         params[1] = 0.0;
         params[2] = alpha;
         return;
     }
-    const double nrm = Ai ? sqrt(fma(alpha, alpha, fma(ai, ai, sigma))) : sqrt(alpha * alpha + sigma);
+    const double nrm = sqrt(nrm2);
     const double beta = alpha >= 0.0 ? -nrm : nrm;
     params[0] = (beta - alpha) / beta;
     if (Ai) {

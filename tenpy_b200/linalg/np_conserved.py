@@ -1815,7 +1815,9 @@ def _block_qr_cgs2(lib, m, n, A, Q, R):
     two skinny GEMMs per pass (projection on the previous vectors), one dot + one scal per column -- and
     ``R = Q^T A`` by one GEMM with the strictly lower triangle dropped.  A column that is linearly dependent on the
     previous ones (norm after projection below ``64 eps`` of its original norm) is replaced by an orthonormalised unit
-    vector, so that `Q` stays an isometry (LAPACK's Householder QR returns an orthonormal completion there, too).
+    vector, so that `Q` stays an isometry (LAPACK's Householder QR returns an orthonormal completion there, too).  Its
+    ``R_jj = q_j^T a_j`` is rounding noise of either sign; where ``R_jj < 0``, ``q_j`` and row j of R change sign, which
+    leaves ``Q R`` unchanged bit for bit and makes ``diag(R) >= 0`` for every column.
 
     Cost model: one host round trip per column (the norm).  This is a functional stand-in on the cold paths
     (`MPS.canonical_form`); a batched Householder kernel is round-2 work (DESIGN.md section 8)."""
@@ -1859,9 +1861,17 @@ def _block_qr_cgs2(lib, m, n, A, Q, R):
         lib.scal(m, 1. / nrm, v)
         Qt[j * m:(j + 1) * m].copy_(v)
     qr_stats['columns'] += k
-    _strided_copy(lib, Qt, 0, Q, 0, [m, k], [1, m], [k, 1])
     Rfull = backend.empty(k * n)
     _gemm(lib, k, n, m, Qt, A, Rfull)
+    diag = backend.empty(k)
+    _strided_copy(lib, Rfull, 0, diag, 0, [k], [n + 1], [1])
+    neg = backend.to_host(diag) < 0.
+    if np.any(neg):                                                 # at replaced columns only
+        sign = backend.to_device(np.where(neg, -1., 1.))
+        for buf, length in ((Qt, m), (Rfull, n)):                   # rows j of Q^T and of R times sign[j]
+            rec = np.array([[0, 1, k, length, 0]], dtype=np.int64)
+            lib.scale_axis(rec, backend.to_device(rec), sign, buf)
+    _strided_copy(lib, Qt, 0, Q, 0, [m, k], [1, m], [k, 1])
     rec = np.zeros((k, 22), dtype=np.int64)                        # row i of R: entries i .. n-1
     i = np.arange(k, dtype=np.int64)
     rec[:, 0] = rec[:, 1] = i * n + i
@@ -1877,11 +1887,12 @@ def qr(a, mode='reduced', inner_labels=[None, None], cutoff=None, pos_diag_R=Fal
     """Q-R decomposition ``a == tensordot(Q, R, axes=1)`` per charge block (reference npc:4139): `Q` an isometry with
     legs ``(a.legs[0], inner.conj())``, `R` upper triangular with legs ``(inner, a.legs[1])``.
 
-    Only ``mode='reduced'`` and ``cutoff=None``.  The diagonal of `R` is non-negative by construction (Householder kernel
-    ``b200_block_qr_f64`` for blocks of up to `QR_HOUSEHOLDER_MAX` rows and columns, Gram-Schmidt :func:`_block_qr_cgs2`
-    above), i.e. the result is the unique decomposition the reference returns for ``pos_diag_R=True`` (for full-rank
-    blocks).  A :class:`ComplexArray` `a` goes through the complex Householder kernel
-    (``b200_block_qr_z``, every block size); `Q` and `R` are then ComplexArrays, the diagonal of `R` real and >= 0."""
+    Only ``mode='reduced'`` and ``cutoff=None``.  The diagonal of `R` is non-negative by construction, on every route and
+    for rank-deficient blocks too (Householder kernel ``b200_block_qr_f64`` for blocks of up to `QR_HOUSEHOLDER_MAX` rows
+    and columns, Gram-Schmidt :func:`_block_qr_cgs2` above), i.e. the result is the unique decomposition the reference
+    returns for ``pos_diag_R=True`` (for full-rank blocks).  A :class:`ComplexArray` `a` goes through the complex
+    Householder kernel (``b200_block_qr_z``, every block size); `Q` and `R` are then ComplexArrays, the diagonal of `R`
+    real and >= 0."""
     if a.rank != 2:
         raise ValueError('expect a matrix!')
     if mode != 'reduced':

@@ -1,8 +1,8 @@
 // Host check of tenpy_b200/csrc/block_qr_core.cuh (test infrastructure): the phases of block_qr_kernel are run for
 // tid = 0..T-1 sequentially, exactly as the CUDA kernel runs them between barriers, for real blocks and for complex blocks
 // (imaginary planes filled); checks A = Q R, Q^H Q = 1, R upper triangular with a real non-negative diagonal, on tall /
-// wide / square / rank deficient / zero-column blocks; then power-of-two equivariance: the QR of 2^e A must give Q bit
-// for bit and R = 2^e R(A) exactly for every e that keeps 2^e A normal.
+// wide / square / rank deficient / zero-column blocks and blocks whose columns span 2^-1050 .. 2^1000; then power-of-two
+// equivariance: the QR of 2^e A must give Q bit for bit and R = 2^e R(A) exactly for every e that keeps 2^e A normal.
 // Run by tests/test_host_qr_scale.py.
 #include <algorithm>
 #include <cmath>
@@ -137,7 +137,7 @@ static int shape_cases(std::mt19937_64 &rng, bool cplx) {
             for (auto &x : v) x += cd(0.0, nd(rng));
     };
     const int shapes[][3] = {{7, 4, 0}, {4, 7, 0}, {5, 5, 0}, {1, 3, 0}, {3, 1, 0}, {33, 20, 0}, {64, 64, 0}, {300, 17, 0},
-                             {12, 8, 3}, {40, 40, 10}, {9, 6, -1}, {1, 1, 0}};
+                             {12, 8, 3}, {40, 40, 10}, {9, 6, -1}, {1, 1, 0}, {7, 5, -2}, {40, 30, -2}, {30, 40, -2}};
     int bad = 0;
     for (auto &sh : shapes) {
         const int m = sh[0], n = sh[1], rank = sh[2], k = std::min(m, n);
@@ -154,14 +154,26 @@ static int shape_cases(std::mt19937_64 &rng, bool cplx) {
                 }
         } else {
             gaussian(A0);
-            if (rank < 0)                                 // an exactly zero column
+            if (rank == -1)                               // an exactly zero column
                 for (int i = 0; i < m; ++i) A0[(size_t)i * n + 2] = 0.0;
+            if (rank == -2) {                             // columns scaled by 2^1000 .. 2^-1050: after the block scaling
+                const int col_exp[] = {1000, 480, -1050, 470, -25, 490, 0, 475, -537};   // squares subnormal or zero
+                for (int i = 0; i < m; ++i)
+                    for (int j = 0; j < n; ++j) {
+                        const int e = col_exp[j % 9];
+                        A0[(size_t)i * n + j] = cd(std::ldexp(A0[(size_t)i * n + j].real(), e),
+                                                   std::ldexp(A0[(size_t)i * n + j].imag(), e));
+                    }
+            }
         }
         std::vector<double> Rr, Ri, Qr, Qi;
         qr_block(A0, m, n, cplx, Rr, Ri, Qr, Qi);
         auto R = [&](int i, int j) { return cd(Rr[(size_t)i * n + j], Ri[(size_t)i * n + j]); };
         auto Q = [&](int i, int j) { return cd(Qr[(size_t)i * k + j], Qi[(size_t)i * k + j]); };
         double rec = 0.0, orth = 0.0, low = 0.0, mindiag = 1e300, imdiag = 0.0, amax = 0.0;
+        bool finite = true;
+        for (size_t i = 0; i < Qr.size(); ++i) finite = finite && std::isfinite(Qr[i]) && std::isfinite(Qi[i]);
+        for (size_t i = 0; i < Rr.size(); ++i) finite = finite && std::isfinite(Rr[i]) && std::isfinite(Ri[i]);
         for (auto a : A0) amax = std::max(amax, std::abs(a));
         for (int i = 0; i < m; ++i)
             for (int j = 0; j < n; ++j) {
@@ -182,8 +194,8 @@ static int shape_cases(std::mt19937_64 &rng, bool cplx) {
         }
         printf("%s%3d x %3d rank %2d: |QR-A| %.2e  |QtQ-1| %.2e  lower %.1e  min diag %.2e\n", cplx ? "complex " : "", m, n,
                rank, rec / std::max(amax, 1e-300), orth, low, mindiag);
-        if (!(rec <= 1e-13 * std::max(amax, 1e-300) * std::max(m, n)) || !(orth < 1e-13) || low != 0.0 || !(mindiag >= 0.0) ||
-            imdiag != 0.0)
+        if (!finite || !(rec <= 1e-13 * std::max(amax, 1e-300) * std::max(m, n)) || !(orth < 1e-13) || low != 0.0 ||
+            !(mindiag >= 0.0) || imdiag != 0.0)
             ++bad;
     }
     return bad;

@@ -103,6 +103,13 @@ def _put_block(planes, off, blk):
         plane.numpy()[off:off + blk.size] = part(blk).reshape(-1)
 
 
+def _ldexp(blk, e):
+    """blk * 2^e, part by part for a complex block"""
+    if np.iscomplexobj(blk):
+        return np.ldexp(blk.real, e) + 1.j * np.ldexp(blk.imag, e)
+    return np.ldexp(blk, e)
+
+
 def fro_norm(blk):
     """|blk|_F without over- or underflow (the kernels scale every block by a power of two first)"""
     amax = np.max(np.abs(blk), initial=0.)
@@ -309,14 +316,21 @@ class FakeDeviceLib:
 
     def _qr(self, m, n, a_off, q_off, r_off, A, Q, R):
         """numpy QR, R with a real non-negative diagonal: the phase (for a real block the sign) of each diagonal entry
-        moves into the column of Q"""
+        moves into the column of Q.  Like the kernel, it factors 2^-e A, 2^e the power of two of max |a_ij| over both
+        planes, and scales R back, so that blocks near the ends of the double range stay finite"""
         for i in range(len(m)):
-            qq, rr = np.linalg.qr(_get_block(A, a_off[i], (int(m[i]), int(n[i]))))
+            blk = _get_block(A, a_off[i], (int(m[i]), int(n[i])))
+            mx = max(np.max(np.abs(blk.real), initial=0.), np.max(np.abs(blk.imag), initial=0.))
+            e = int(np.clip(np.frexp(mx)[1] - 1, -1022, 1022)) if mx > 0. else 0
+            qq, rr = np.linalg.qr(_ldexp(blk, -e))
             d = np.diag(rr)
             ad = np.abs(d)
-            ph = np.where(ad > 0., d / np.where(ad > 0., ad, 1.), 1.)
+            safe = np.where(ad > 0., ad, 1.)
+            ph = np.where(ad > 0., d.real / safe, 1.)          # part by part: a complex division by a subnormal overflows
+            if np.iscomplexobj(d):
+                ph = ph + 1.j * (d.imag / safe)
             _put_block(Q, q_off[i], qq * ph[None, :])
-            _put_block(R, r_off[i], rr * ph.conj()[:, None])
+            _put_block(R, r_off[i], _ldexp(rr * ph.conj()[:, None], e))
 
     def col_sqnorms(self, rows, cols, ld, X, OUT):
         self._count('col_sqnorms')
