@@ -209,6 +209,18 @@ int b200_mid_contract_f64(int64_t K, int64_t N, int64_t outer, int64_t inner, co
 int b200_mid_contract2_f64(int64_t K1, int64_t K2, int64_t N1, int64_t N2, int64_t outer, int64_t inner,
                            const double *M_dev, const double *T1, const double *T2, double *OUT1, double *OUT2,
                            b200_stream_t stream);
+/* complex two-segment version, the same contraction for complex M, T1, T2 in one read of each input.  M (N x K), T1
+ * (outer x K1 x inner), T2 (outer x K2 x inner) and OUT2 (outer x N2 x inner) are planar: the real plane, then the
+ * imaginary plane of the same size, in one buffer.  OUT1 is written as the real 2x2 embedding [[Yr, -Yi], [Yi, Yr]]
+ * (2m x 2w, row-major) of the matrix Y[(o, n / C1), (n % C1, i)], m = outer N1 / C1, w = C1 inner: it is the left
+ * operand of the next GEMM, which then multiplies the stacked planes [Br; Bi] of its right operand and returns a planar
+ * result.  Serves the split-order matvec of complex states in the reference's combine=False contraction order
+ * (mps_common.py:1340): T1 = LP_rest.theta, T2 = theta, OUT1 -> product with RP_rest, OUT2 -> added to the result.
+ * Refused (B200_ERR_ARG): K = K1 + K2 outside 1..32, N = N1 + N2 above 1024, C1 not dividing N1 > 0, or both planes of M
+ * above 48 KB. */
+int b200_mid_contract2_z(int64_t K1, int64_t K2, int64_t N1, int64_t N2, int64_t C1, int64_t outer, int64_t inner,
+                         const double *M_dev, const double *T1, const double *T2, double *OUT1, double *OUT2,
+                         b200_stream_t stream);
 
 /* OUT[c] = sum_r X[r*ld + c]^2 for a row-major (rows x cols) matrix (leverage scores of the null-space
  * completion in np_conserved.svd; no reference counterpart: LAPACK returns a complete basis by itself) */

@@ -64,6 +64,8 @@ _SIGNATURES = {
     'b200_block_qr_worksize': (c_i64, [c_i64, c_i64p, c_i64p]),
     'b200_block_qr_f64': (ctypes.c_int, [c_i64, c_i64p, c_i64p, c_i64p, c_i64p, c_i64p, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp]),
     'b200_mid_contract2_f64': (ctypes.c_int, [c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    'b200_mid_contract2_z': (ctypes.c_int, [c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp,
+                                            c_vp, c_vp]),
     'b200_mid_contract_f64': (ctypes.c_int, [c_i64, c_i64, c_i64, c_i64, c_vp, c_vp, c_vp, c_vp]),
     'b200_ozaki_split_worksize': (c_i64, [c_i64, c_i64, c_i32]),
     'b200_ozaki_split_f64': (ctypes.c_int, [c_i64, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp, c_i64, c_vp]),
@@ -386,6 +388,14 @@ class DeviceLib:
             self._check(self.c.b200_mid_contract2_f64(int(K1), int(K2), int(N1), int(N2), int(outer), int(inner),
                                                       _ptr(M), _ptr(T1), _ptr(T2), _ptr(OUT1), _ptr(OUT2),
                                                       self.stream()))
+
+    def mid_contract2_z(self, K1, K2, N1, N2, C1, outer, inner, M, T1, T2, OUT1, OUT2):
+        """the complex form of :meth:`mid_contract2`: planar M, T1, T2, OUT2; OUT1 the real embedding of
+        Y[(o, n / C1), (n % C1, i)] (include/b200npc.h)"""
+        with _Prof(self, 'move'):
+            self._check(self.c.b200_mid_contract2_z(int(K1), int(K2), int(N1), int(N2), int(C1), int(outer), int(inner),
+                                                    _ptr(M), _ptr(T1), _ptr(T2), _ptr(OUT1), _ptr(OUT2),
+                                                    self.stream()))
 
     # -- decompositions
     def _svd_call(self, fn, worksize, m, n, a_off, u_off, s_off, vt_off, A, U, S, VT):

@@ -45,6 +45,10 @@ _TWO_SITE_CHAINS = {
 }
 
 
+def _is_complex(x):
+    return np.dtype(x.dtype).kind == 'c'
+
+
 _EYE_CACHE = {}
 
 
@@ -165,6 +169,54 @@ def _get_RHeff(env, i, eff_H):
     return env._contract_RHeff(i)
 
 
+_DENSE_PLANS = {}
+
+
+def _dense_plan(m, n, k):
+    """the grouped-GEMM plan of one dense product (m x k) . (k x n) at offset 0 of raw buffers, kept per shape"""
+    from .. import backend
+    lib = backend.get_lib()
+    hit = _DENSE_PLANS.get((m, n, k))
+    if hit is None or hit[0] is not lib:
+        if len(_DENSE_PLANS) > 64:
+            _DENSE_PLANS.clear()
+        q = np.zeros((1, 2), np.int64)
+        hit = _DENSE_PLANS[(m, n, k)] = (lib, lib.tdot_plan(q, q, 1, [m], [k], [0], [k], [n], [0]))
+    return hit[1]
+
+
+def _real_embedding(a):
+    """the real 2x2 embedding ``[[Ar, -Ai], [Ai, Ar]]`` (row-major, 2m x 2k) of the one-block tensor `a` (real or complex)
+    read as the matrix [(leg 0, leg 1), leg 2]"""
+    from .. import backend
+    lay, planes = npc._planes(a)
+    m, k = a.shape[0] * a.shape[1], a.shape[2]
+    o = int(lay.offsets[0])
+    ar = planes[0][o:o + m * k].view(m, k)
+    E = backend.empty(4 * m * k) if len(planes) == 2 else backend.zeros(4 * m * k)
+    Ev = E.view(2, m, 2, k)
+    Ev[0, :, 0].copy_(ar)
+    Ev[1, :, 1].copy_(ar)
+    if len(planes) == 2:
+        ai = planes[1][o:o + m * k]
+        Ev[1, :, 0].copy_(ai.view(m, k))
+        neg = ai.clone()
+        backend.get_lib().scal(m * k, -1., neg)
+        Ev[0, :, 1].copy_(neg.view(m, k))
+    return E
+
+
+def _stacked_planes(a):
+    """the planes of the one-block tensor `a` (real or complex) stacked in one buffer ``[Ar; Ai]``"""
+    from .. import backend
+    lay, planes = npc._planes(a)
+    n, o = int(lay.sizes[0]), int(lay.offsets[0])
+    S = backend.empty(2 * n) if len(planes) == 2 else backend.zeros(2 * n)
+    for j, p in enumerate(planes):
+        S[j * n:(j + 1) * n].copy_(p[o:o + n])
+    return S
+
+
 class IdentityEnvRejected(Exception):
     """raised by `SplitOrderMatvec.deferred_check` when the environments turn out not to have identity components: the
     caller restarts its iteration, the effective Hamiltonian has switched the shortcut off"""
@@ -187,7 +239,11 @@ class SplitOrderMatvec:
 
     The shapes alone choose how ``W0.W1`` is applied: to dense tensors (one block) with ``K = D d^2 <= 32`` contracted
     rows (``K1 + K2 = (D-1) d^2 + d^2`` without the identity components) by the streaming kernel b200_mid_contract(2)_f64,
-    which keeps the layout; otherwise by `npc.tensordot` (two block transpositions and a skinny GEMM)."""
+    which keeps the layout; otherwise by `npc.tensordot` (two block transpositions and a skinny GEMM).
+
+    Complex theta and MPOs take the same routes with the same rule for ``'auto'`` (the largest block of either plane of
+    theta): with charges `npc.tensordot` composes each complex product of real ones; dense, with the packed complex
+    Krylov vector, the replayed kernel sequence uses b200_mid_contract2_z (see :meth:`_dense_z_run`)."""
     SPLIT_MIN_BLOCK = 1 << 20
     matvec_order = 'auto'
     # skip the identity components of the environments in the split-order matvec (see _identity_env_setup): host logic on
@@ -208,11 +264,20 @@ class SplitOrderMatvec:
     _M_id = _N1 = _fused_legs = _RP_rest_t = None      # fused identity route, see _bind_fused_identity
     _dense_recipe = None                               # replayed kernel sequence, see _dense_recipe_bind
     _dense_recipe_off = False
+    _dense_z = None                                    # its complex form, see _dense_z_bind
+    _dense_z_off = False
 
     def _use_split(self, theta):
         if self.matvec_order == 'auto':
-            sizes = theta._layout.sizes
-            return len(sizes) > 0 and int(sizes.max()) >= self.SPLIT_MIN_BLOCK
+            # a complex theta: the block tables of its planes (a block of the union of the two is a block of one of them).
+            # Complex theta with charges keep the combined order: on the H100 the split order through the composed real
+            # products was 0.77x / 0.90x / 0.97x the speed of the combined order for the DM chain (Sz) at chi = 256 / 512 /
+            # 1024 (DESIGN.md section 3.3); one-block theta take the dense kernel sequence from SPLIT_MIN_BLOCK on.
+            parts = (theta.re, theta.im) if _is_complex(theta) else (theta,)
+            sizes = [int(p._layout.sizes.max()) for p in parts if p._layout.nblocks]
+            if len(parts) == 2 and max(p._layout.nblocks for p in parts) > 1:
+                return False
+            return len(sizes) > 0 and max(sizes) >= self.SPLIT_MIN_BLOCK
         return self.matvec_order == 'split'
 
     def _combine_result(self, out, labels):
@@ -224,11 +289,18 @@ class SplitOrderMatvec:
         """``LP . theta . (W0 W1) . RP`` on the split legs; interface (labels, pipes) of the combined matvec."""
         if self._W01 is None:
             self._W01 = npc.tensordot(self.W0, self.W1, axes=['wR', 'wL'])   # wL p0 p0* p1 p1* wR  (D^2 d^4 numbers)
-        rec = self._dense_recipe
-        if rec is None and not self._dense_recipe_off and self.identity_env:
-            rec = self._dense_recipe_from_cache(theta)
-        if rec is not None and theta._layout is rec['theta_lay'] and theta._labels == rec['labels']:
-            return self._dense_recipe_run(theta, rec)
+        if _is_complex(theta):
+            # complex theta: the dense kernel sequence if it applies (_dense_z_run), else the Array-level routes below,
+            # whose products npc.tensordot composes of real ones
+            out = self._dense_z_run(theta) if self.identity_env and self._id_env is not False else None
+            if out is not None:
+                return out
+        else:
+            rec = self._dense_recipe
+            if rec is None and not self._dense_recipe_off and self.identity_env:
+                rec = self._dense_recipe_from_cache(theta)
+            if rec is not None and theta._layout is rec['theta_lay'] and theta._labels == rec['labels']:
+                return self._dense_recipe_run(theta, rec)
         th = theta.split_legs(['(vL.p0)', '(p1.vR)'], _view=True)            # vL p0 p1 vR (read only here)
         if self.identity_env and self._id_env is not False:
             try:
@@ -272,7 +344,7 @@ class SplitOrderMatvec:
         for out, lim in pending:
             if not backend.read_scalar(out) <= lim:
                 self._id_env = False
-                self._dense_recipe = None
+                self._dense_recipe = self._dense_z = None
                 self._dense_recipe_off = True
                 SplitOrderMatvec.stats['identity_env_bonds'] -= 1
                 SplitOrderMatvec.stats['identity_env_rejected'] += 1
@@ -293,16 +365,22 @@ class SplitOrderMatvec:
             comp = part.take_slice(idx, lab)
             if np.any(comp.qtotal != 0):
                 return False
-            eye = _cached_eye(comp)
+            eye = _cached_eye(comp.re if _is_complex(comp) else comp)
             if comp.legs[1].qconj != eye.legs[1].qconj:
                 return False
-            diff = comp - eye
-            if self.identity_check == 'deferred' and diff._layout.nblocks:
+            diff = comp - eye                    # complex: Re LP[IdL] - 1 and Im LP[IdL], both have to vanish
+            planes = [p for p in ((diff.re, diff.im) if _is_complex(diff) else (diff,)) if p._layout.nblocks]
+            if self.identity_check == 'deferred' and planes:
                 # |LP[IdL] - 1|^2 stays on the device; it is read together with the Lanczos scalars (the next unavoidable
                 # synchronisation, `deferred_check`), so the set-up costs no round trip of its own
                 from .. import backend
+                lib = backend.get_lib()
                 out = backend.empty(1)
-                backend.get_lib().dot(diff._layout.size, diff._buf, diff._buf, backend.dot_scratch(), out)
+                lib.dot(planes[0]._layout.size, planes[0]._buf, planes[0]._buf, backend.dot_scratch(), out)
+                for p in planes[1:]:                                              # + |Im LP[IdL]|^2
+                    sq = backend.empty(1)
+                    lib.dot(p._layout.size, p._buf, p._buf, backend.dot_scratch(), sq)
+                    lib.axpy(1, 1., sq, out)
                 pending.append((out, (1.e-11 * np.sqrt(comp.shape[0]))**2))
             elif not npc.norm(diff) <= 1.e-11 * np.sqrt(comp.shape[0]):
                 return False
@@ -449,11 +527,130 @@ class SplitOrderMatvec:
         res._buf = out
         return res
 
+    # The same sequence for a complex theta, on real kernels with doubled dimensions.  theta is the packed Krylov vector
+    # of the complex Lanczos (krylov_based._pack): one buffer [theta_r; theta_i], i.e. a (2 chi_l) x (d0 d1 chi_r) matrix.
+    #   t1 = [[Lr, -Li], [Li, Lr]] . [theta_r; theta_i]               one DMMA product, result planar [t1_r; t1_i]
+    #   Y_emb, Y_id = (W0 W1) . [t1; theta]                             b200_mid_contract2_z: Y_emb = [[Yr, -Yi], [Yi, Yr]]
+    #   out = Y_emb . [Rr; Ri]                                          one DMMA product, result planar [out_r; out_i]
+    #   out += Y_id                                                     one axpy over both planes
+    # The embedding of LP_rest and the stacked planes of RP_rest are constants of the bond (made once, like the
+    # int8 digit planes of the real route); the kernel geometry (plans, the complex W0 W1 matrix) is kept in the per-bond
+    # cache on the MPO.  Mixed dtypes take the same sequence when theta is complex (a real LP, RP or W0 W1 gets a zero
+    # imaginary plane); a real theta with a complex MPO takes the Array-level route (npc.tensordot composes the complex
+    # products of real ones), as does every theta that is not a packed, unpadded one-block vector.
+    def _dense_z_run(self, theta):
+        """the dense complex kernel sequence for `theta`; None if it does not apply (then the Array-level route)"""
+        rec = self._dense_z
+        if rec is None:
+            if self._dense_z_off:
+                return None
+            try:
+                rec = self._dense_z_bind(theta)
+            except Exception as e:       # as for the real routes: a shortcut must never take the matvec down
+                import logging
+                logging.getLogger(__name__).warning('dense complex route disabled for bond %d: %r', self.i0, e)
+                rec = None
+            if rec is None:
+                self._dense_z_off = True
+                return None
+        if not self._dense_z_fits(theta, rec) or self._id_env is False:
+            return None
+        from .. import backend
+        lib = backend.get_lib()
+        s = npc.OZAKI['slices_matvec']
+        kbuf = theta._kbuf
+        t1 = backend.empty(rec['n_t1'])
+        npc._raw_product(lib, rec['E'], kbuf, rec['g1'], rec['plan1'], t1, s)
+        y_emb, y_id = backend.empty(rec['n_emb']), backend.empty(2 * rec['n'])
+        K1, K2, N1, N2, C1, chi_l, chi_r = rec['mid']
+        lib.mid_contract2_z(K1, K2, N1, N2, C1, chi_l, chi_r, rec['M'], t1, kbuf, y_emb, y_id)
+        n = rec['n']
+        out = backend.empty(2 * n)
+        npc._raw_product(lib, y_emb, rec['R'], rec['g2'], rec['plan2'], out, s)
+        lib.axpy(2 * n, 1., y_id, out)
+        res = npc._from_planes(theta.legs, theta.qtotal, rec['theta_lay'], (out[:n], out[n:]), theta.get_leg_labels())
+        res._kbuf = out
+        return res
+
+    @staticmethod
+    def _dense_z_fits(theta, rec):
+        """`theta` is a packed complex vector on the recorded one-block layout: its planes are the two halves of `_kbuf`"""
+        kbuf = getattr(theta, '_kbuf', None)
+        if kbuf is None or not hasattr(theta, 're') or theta._labels != rec['labels']:
+            return False
+        lay, n = rec['theta_lay'], rec['n']
+        re, im = theta.re, theta.im
+        return (re._layout is lay or re._layout.same_blocks(lay)) and (im._layout is lay or im._layout.same_blocks(lay)) \
+            and kbuf.numel() == 2 * n and re._buf.data_ptr() == kbuf.data_ptr() and \
+            im._buf.data_ptr() == kbuf[n:].data_ptr()
+
+    def _dense_z_bind(self, theta):
+        """first complex matvec of the bond: check that the dense sequence applies, make the bond's constants and take the
+        kernel geometry from the cache on the MPO (recorded there on the first visit of the bond)"""
+        if not hasattr(theta, 're') or getattr(theta, '_kbuf', None) is None:
+            return None
+        lay = theta.re._layout
+        if lay.nblocks != 1 or lay.has_padding or int(lay.offsets[0]) != 0 or \
+                theta.get_leg_labels() != ['(vL.p0)', '(p1.vR)']:
+            return None
+        if self._W01.stored_blocks != 1 or not self._identity_env_setup():
+            return None
+        rec = {'theta_lay': lay, 'labels': list(theta._labels), 'n': int(lay.size)}
+        if not self._dense_z_fits(theta, rec):
+            return None
+        th = theta.re.split_legs(['(vL.p0)', '(p1.vR)'], _view=True)
+        if th._buf.data_ptr() != theta.re._buf.data_ptr() or th.get_leg_labels() != ['vL', 'p0', 'p1', 'vR']:
+            return None                  # the pipes are not a plain reshape of the buffer
+        chi_l, d0, d1, chi_r = th.shape
+        L = self._LP_rest.transpose(['vR*', 'wR', 'vR'])
+        R = self._RP_rest.transpose(['wL', 'vL', 'vL*'])
+        if L.stored_blocks != 1 or R.stored_blocks != 1:
+            return None
+        Dl, Dr = L.shape[1], R.shape[0]
+        if L.shape != (chi_l, Dl, chi_l) or R.shape != (Dr, chi_r, chi_r):
+            return None
+        K1, K2, N1, N2 = Dl * d0 * d1, d0 * d1, Dr * d0 * d1, d0 * d1
+        if K1 + K2 > 32 or 2 * (N1 + N2) * (K1 + K2) * 8 > 48 * 1024:
+            return None
+        ent = self._mpo_cache
+        geom = ent.get('z_geom')
+        shape = (chi_l, Dl, Dr, d0, d1, chi_r)
+        if geom is None or geom['shape'] != shape:           # first visit of the bond, or its bond dimensions changed
+            geom = ent['z_geom'] = {'shape': shape, 'M': None if geom is None else geom['M']}
+            m1, m2, nc = chi_l * Dl, chi_l * d0 * d1, d0 * d1 * chi_r
+            geom['g1'], geom['g2'] = (2 * m1, nc, 2 * chi_l), (2 * m2, chi_r, 2 * Dr * chi_r)
+            geom['plan1'], geom['plan2'] = _dense_plan(*geom['g1']), _dense_plan(*geom['g2'])
+        if geom['M'] is None:
+            geom['M'] = self._w01_planes_identity_last()
+        rec.update(E=_real_embedding(L), R=_stacked_planes(R), M=geom['M'], g1=geom['g1'], g2=geom['g2'],
+                   plan1=geom['plan1'], plan2=geom['plan2'], mid=(K1, K2, N1, N2, Dr, chi_l, chi_r),
+                   n_t1=2 * chi_l * Dl * d0 * d1 * chi_r, n_emb=4 * chi_l * d0 * d1 * Dr * chi_r)
+        self._dense_z = rec
+        return rec
+
+    def _w01_planes_identity_last(self):
+        """``W0 W1`` as the planar matrix [Mr | Mi] of [(p0' p1' wR), (wL p0 p1)] with the identity components at the end of
+        both MPO index groups (as `M_id` of the real route, :meth:`_apply_W01_fused_identity`)"""
+        from .. import backend
+        H = self._H_mpo
+        IdL, IdR = H.get_IdL(self.i0), H.get_IdR(self.i0 + 1)
+        W = self._W01.transpose(['p0', 'p1', 'wR', 'wL', 'p0*', 'p1*']).to_ndarray()
+        d0, d1, D_r, D_l = W.shape[0], W.shape[1], W.shape[2], W.shape[3]
+        rest_r = [x for x in range(D_r) if x != IdR]
+        rest_l = [x for x in range(D_l) if x != IdL]
+        rows = np.concatenate([W[:, :, rest_r].reshape(d0 * d1 * len(rest_r), D_l, d0, d1),
+                               W[:, :, IdR].reshape(d0 * d1, D_l, d0, d1)], axis=0)
+        M = np.concatenate([rows[:, rest_l].reshape(rows.shape[0], -1), rows[:, IdL].reshape(rows.shape[0], -1)], axis=1)
+        return backend.to_device(np.concatenate([M.real.reshape(-1), np.imag(M).reshape(-1)]))
+
     @staticmethod
     def _split_t2_views(t2):
         """``t2`` (legs ``vR*, vR, p0, wR, p1``) with the MPO leg in two sectors [others, IdR] and no other sector structure: the two
         stored blocks ARE the two components.  Returns read-only views ``(t2_rest, direct)`` sharing the packed buffer
-        (`direct` without its unit MPO leg), or None if the structure is different (charged tensors)."""
+        (`direct` without its unit MPO leg), or None if the structure is different (charged tensors) or `t2` is complex
+        (then the two components are taken by `take_slice` / `iproject`, plane by plane)."""
+        if _is_complex(t2):
+            return None
         lay = t2._layout
         ax = t2.get_leg_index('wR')
         leg = t2.legs[ax]
@@ -490,6 +687,8 @@ class SplitOrderMatvec:
         are read once, both outputs come out in the layout their consumer wants.  Dense (one block) only; None if not
         applicable."""
         from .. import backend
+        if _is_complex(t1) or _is_complex(th) or _is_complex(self._W01):
+            return None                  # complex operands: the dense kernel sequence _dense_z_run, or npc.tensordot
         if t1._layout.nblocks != 1 or th._layout.nblocks != 1 or self._W01._layout.nblocks != 1 or \
                 t1.get_leg_labels() != ['vR*', 'wR', 'p0', 'p1', 'vR'] or th.get_leg_labels() != ['vL', 'p0', 'p1', 'vR']:
             return None
@@ -535,6 +734,8 @@ class SplitOrderMatvec:
         returns None if not applicable."""
         from .. import backend
         W01 = self._W01
+        if _is_complex(th) or _is_complex(W01):
+            return None                  # complex operands: W0 W1 by npc.tensordot
         if th._layout.nblocks != 1 or W01._layout.nblocks != 1 or th.get_leg_labels() != ['vR*', 'wR', 'p0', 'p1', 'vR']:
             return None
         if self._W01_mat is None:
@@ -583,11 +784,10 @@ class TwoSiteH(SplitOrderMatvec):
             self.combine_Heff(env)
 
     def matvec(self, theta):
-        """Apply the effective Hamiltonian to `theta` (reference mps_common.py:1321).  A complex `theta` or MPO takes the
-        combined (or plain) order: the split-order routes and their per-bond caches are real-only."""
+        """Apply the effective Hamiltonian to `theta` (reference mps_common.py:1321); real and complex `theta` and MPOs
+        alike (the routes of :class:`SplitOrderMatvec`)."""
         labels = theta.get_leg_labels()
-        if self.combine and np.dtype(self.dtype).kind != 'c' and np.dtype(theta.dtype).kind != 'c' and \
-                self._use_split(theta):
+        if self.combine and self._use_split(theta):
             return self._matvec_split(theta, labels)
         chain, relabel = _TWO_SITE_CHAINS['combined' if self.combine else 'plain']
         return _apply_chain(self, theta, chain, relabel).itranspose(labels)

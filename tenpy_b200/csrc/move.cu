@@ -131,6 +131,25 @@ __global__ void __launch_bounds__(MV_THREADS) mid_contract2_kernel(int K1, int K
         midc::column2<KMAX>(o, i, K1, K2, N1, N2, inner, sM, T1, T2, OUT1, OUT2);
 }
 
+// complex form (midc::column2_z): both planes of M in shared memory, one thread per (o, i) column
+template <int KMAX>
+__global__ void __launch_bounds__(MV_THREADS) mid_contract2_z_kernel(int K1, int K2, int N1, int N2, int C1,
+                                                                     int64_t outer, int64_t inner,
+                                                                     const double *__restrict__ M,
+                                                                     const double *__restrict__ T1,
+                                                                     const double *__restrict__ T2,
+                                                                     double *__restrict__ OUT1,
+                                                                     double *__restrict__ OUT2) {
+    extern __shared__ double sM[];
+    const int NK = (N1 + N2) * (K1 + K2);
+    for (int idx = threadIdx.x; idx < 2 * NK; idx += blockDim.x) sM[idx] = M[idx];
+    __syncthreads();
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= inner) return;
+    for (int64_t o = blockIdx.y; o < outer; o += gridDim.y)
+        midc::column2_z<KMAX>(o, i, K1, K2, N1, N2, C1, outer, inner, sM, sM + NK, T1, T2, OUT1, OUT2);
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -150,6 +169,29 @@ extern "C" int b200_mid_contract2_f64(int64_t K1, int64_t K2, int64_t N1, int64_
         mid_contract2_kernel<16><<<dim3(gx, gy), MV_THREADS, smem, (cudaStream_t)stream>>>((int)K1, (int)K2, (int)N1, (int)N2, outer, inner, M_dev, T1, T2, OUT1, OUT2);
     else
         mid_contract2_kernel<32><<<dim3(gx, gy), MV_THREADS, smem, (cudaStream_t)stream>>>((int)K1, (int)K2, (int)N1, (int)N2, outer, inner, M_dev, T1, T2, OUT1, OUT2);
+    B200_CHECK_LAUNCH();
+    return B200_OK;
+}
+
+extern "C" int b200_mid_contract2_z(int64_t K1, int64_t K2, int64_t N1, int64_t N2, int64_t C1, int64_t outer,
+                                    int64_t inner, const double *M_dev, const double *T1, const double *T2, double *OUT1,
+                                    double *OUT2, b200_stream_t stream) {
+    const int64_t K = K1 + K2, N = N1 + N2;
+    if (outer <= 0 || inner <= 0 || N <= 0) return B200_OK;
+    if (K1 < 0 || K2 < 0 || N1 < 0 || N2 < 0 || K <= 0 || K > 32 || N > 1024)
+        return set_error(B200_ERR_ARG, "mid_contract2_z: K=%lld (1..32), N=%lld (<=1024)", (long long)K, (long long)N);
+    if (N1 > 0 && (C1 <= 0 || N1 % C1 != 0))
+        return set_error(B200_ERR_ARG, "mid_contract2_z: C1=%lld does not divide N1=%lld", (long long)C1, (long long)N1);
+    const unsigned gx = (unsigned)((inner + MV_THREADS - 1) / MV_THREADS);
+    const unsigned gy = (unsigned)(outer < 65535 ? outer : 65535);
+    const size_t smem = (size_t)(2 * N * K) * sizeof(double);
+    if (smem > 48 * 1024)
+        return set_error(B200_ERR_ARG, "mid_contract2_z: matrix %lld x %lld too large", (long long)N, (long long)K);
+    const int c1 = N1 > 0 ? (int)C1 : 1;
+    if (K <= 16)
+        mid_contract2_z_kernel<16><<<dim3(gx, gy), MV_THREADS, smem, (cudaStream_t)stream>>>((int)K1, (int)K2, (int)N1, (int)N2, c1, outer, inner, M_dev, T1, T2, OUT1, OUT2);
+    else
+        mid_contract2_z_kernel<32><<<dim3(gx, gy), MV_THREADS, smem, (cudaStream_t)stream>>>((int)K1, (int)K2, (int)N1, (int)N2, c1, outer, inner, M_dev, T1, T2, OUT1, OUT2);
     B200_CHECK_LAUNCH();
     return B200_OK;
 }

@@ -100,7 +100,6 @@ def fast_two_site_engine():
     own extension point ``EffectiveH``.  Call after :func:`install`."""
     if not installed():
         raise RuntimeError('call tenpy_b200.dropin.install() first')
-    import numpy as np
     from tenpy.algorithms import dmrg as ref_dmrg
     from tenpy.algorithms import mps_common as ref_common
     from .algorithms.mps_common import SplitOrderMatvec
@@ -115,9 +114,8 @@ def fast_two_site_engine():
             self._H_mpo = env.H
 
         def matvec(self, theta):
-            # the split-order routes are real-only: a complex theta or MPO takes the reference's order
-            if self.combine and np.dtype(self.dtype).kind != 'c' and np.dtype(theta.dtype).kind != 'c' and \
-                    self._use_split(theta):
+            # real and complex theta and MPOs alike (SplitOrderMatvec)
+            if self.combine and self._use_split(theta):
                 return self._matvec_split(theta, theta.get_leg_labels())
             return super().matvec(theta)
 
