@@ -158,6 +158,17 @@ int b200_lanczos_update_dev_f64(int64_t n, const double *alpha_dev, const double
                                 const double *V0, double *W, double *scratch_dev, double *out_dev,
                                 b200_stream_t stream);
 int b200_scal_rsqrt_dev_f64(int64_t n, const double *norm2_dev, double *X, b200_stream_t stream);
+/* Krylov result assembly with complex coefficients (krylov_based.py:160 `_calc_result_full`, used for the Lanczos time
+ * evolution): OUT = sum_{k < nvec} c_k v_k with c_k = coef_dev[2k] + i coef_dev[2k+1].  v_k is one plane of n doubles
+ * (a real Krylov vector, in_planes = 1) or the planes [re; im] of 2n doubles (a packed complex one, in_planes = 2);
+ * OUT is always the packed complex vector [re; im] of 2n doubles.  V_dev / coef_dev: the pointer table and the
+ * coefficients in device memory; V_host: the same pointer table on the host, read for the argument checks only.  One
+ * thread per element, FP64 accumulation in the order of the table.  Per complex output element it reads
+ * 8 * in_planes * nvec bytes and writes 16 (the same result by axpy passes reads and rewrites OUT three times per vector).
+ * Refused (B200_ERR_ARG, nothing launched): nvec outside 1..64, in_planes not 1 or 2, n < 0, a null pointer, OUT
+ * overlapping a v_k.  n = 0 launches nothing. */
+int b200_krylov_combine_f64(int64_t n, int64_t nvec, int64_t in_planes, const double *const *V_dev,
+                            const double *const *V_host, const double *coef_dev, double *OUT, b200_stream_t stream);
 
 /* ---- block data movement ------------------------------------------------------------------------- */
 /* Strided N-d block copies: dst[doff + sum_i idx_i*dstride_i] = src[soff + sum_i idx_i*sstride_i].

@@ -57,6 +57,7 @@ _SIGNATURES = {
     'b200_lanczos_update_f64': (ctypes.c_int, [c_i64, c_f64, c_vp, c_f64, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'b200_lanczos_update_dev_f64': (ctypes.c_int, [c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     'b200_scal_rsqrt_dev_f64': (ctypes.c_int, [c_i64, c_vp, c_vp, c_vp]),
+    'b200_krylov_combine_f64': (ctypes.c_int, [c_i64, c_i64, c_i64, c_vp, c_i64p, c_vp, c_vp, c_vp]),
     'b200_copy_blocks_f64': (ctypes.c_int, [c_i64, c_vp, c_i64p, c_vp, c_vp, c_vp]),
     'b200_take_blocks_f64': (ctypes.c_int, [c_i64, c_vp, c_i64p, c_vp, c_vp, c_vp, c_vp]),
     'b200_scale_axis_f64': (ctypes.c_int, [c_i64, c_vp, c_i64p, c_vp, c_vp, c_vp]),
@@ -356,6 +357,14 @@ class DeviceLib:
         """x *= 1 / sqrt(norm2_dev[0])"""
         with _Prof(self, 'blas1'):
             self._check(self.c.b200_scal_rsqrt_dev_f64(n, _ptr(norm2_dev), _ptr(X), self.stream()))
+
+    def krylov_combine(self, n, in_planes, ptr_host, ptr_dev, coef_dev, OUT):
+        """OUT[:2n] = sum_k c_k v_k, c_k = coef_dev[2k] + i coef_dev[2k+1]: `ptr_host` the int64 addresses of the v_k (one
+        plane of n or two of 2n doubles, `in_planes`), `ptr_dev` the same table on the device (include/b200npc.h)"""
+        ph, php = _i64(ptr_host)
+        with _Prof(self, 'blas1'):
+            self._check(self.c.b200_krylov_combine_f64(int(n), len(ph), int(in_planes), _ptr(ptr_dev), php,
+                                                       _ptr(coef_dev), _ptr(OUT), self.stream()))
 
     # -- data movement
     def copy_blocks(self, task_host, task_dev, SRC, DST):

@@ -1,6 +1,6 @@
-"""The two-site effective Hamiltonian and the density-matrix mixer.
+"""The zero-, one- and two-site effective Hamiltonians and the density-matrix mixer.
 
-Host-side mirror of the reference ``tenpy/algorithms/mps_common.py``: `TwoSiteH` (:1245; `matvec` :1321,
+Host-side mirror of the reference ``tenpy/algorithms/mps_common.py``: `ZeroSiteH` (:1440), `TwoSiteH` (:1245; `matvec` :1321,
 `combine_Heff` :1350, `combine_theta` :1374, `update_LP` :1421, `update_RP` :1430) and
 `DensityMatrixMixer` (:1903; `mix_rho` :1972, `svd_from_rho` :2029, `_mix_LR` :1846).  The contraction
 sequences are the reference's; each ``npc.tensordot`` is one grouped FP64 tensor-core GEMM launch.
@@ -12,7 +12,7 @@ import numpy as np
 from ..linalg import np_conserved as npc
 from ..linalg.truncation import truncate
 
-__all__ = ['OneSiteH', 'TwoSiteH', 'Mixer', 'DensityMatrixMixer', 'SubspaceExpansion']
+__all__ = ['ZeroSiteH', 'OneSiteH', 'TwoSiteH', 'Mixer', 'DensityMatrixMixer', 'SubspaceExpansion']
 
 
 def _apply_chain(obj, theta, chain, relabel):
@@ -145,6 +145,33 @@ class OneSiteH:
             env.set_RP(i, RP, age=env.get_RP_age(i + 1) + 1)
         else:
             env.get_RP(i, store=True)
+
+
+class ZeroSiteH:
+    r"""Effective Hamiltonian ``LP--RP`` acting on the bond matrix left of site `i0` (reference mps_common.py:1440): the
+    backward step of the single-site TDVP.  `theta` has the labels ``'vL', 'vR'``."""
+    length = 0
+    acts_on = ['vL', 'vR']
+
+    def __init__(self, env, i0):
+        self.i0 = i0
+        self.LP = env.get_LP(i0)
+        self.RP = env.get_RP(i0 - 1)
+        self.dtype = env.H.dtype
+        self.N = self.LP.get_leg('vR').ind_len * self.RP.get_leg('vL').ind_len
+
+    def matvec(self, theta):
+        """``LP . theta . RP`` (reference mps_common.py:1497)."""
+        labels = theta.get_leg_labels()
+        theta = npc.tensordot(self.LP, theta, axes=['vR', 'vL'])
+        theta = npc.tensordot(theta, self.RP, axes=[['wR', 'vR'], ['wL', 'vL']])
+        theta.ireplace_labels(['vR*', 'vL*'], ['vL', 'vR'])
+        return theta.itranspose(labels)
+
+    def to_matrix(self):
+        """Contract `self` to a 2D Array (small systems only; reference mps_common.py:1518)."""
+        contr = npc.tensordot(self.LP, self.RP, axes=['wR', 'wL'])
+        return contr.combine_legs([['vR*', 'vL*'], ['vR', 'vL']], qconj=[+1, -1])
 
 
 def _get_LHeff(env, i, eff_H):

@@ -171,6 +171,42 @@ __global__ void __launch_bounds__(B1_THREADS) dot_seg_kernel(const int64_t *__re
     if (threadIdx.x == 0) partial[(int64_t)blockIdx.y * gridDim.x + blockIdx.x] = s;
 }
 
+// out = sum_k c_k v_k for complex c_k (coef[2k] + i coef[2k+1]); v_k one plane (real, in_planes = 1) or the planes
+// [re; im] of a packed complex vector (in_planes = 2); out is always [re; im].  One thread per element, the sum over k in
+// the order of the table, so that a result does not depend on the launch geometry.
+constexpr int KC_MAX_VEC = 64;
+
+__global__ void __launch_bounds__(B1_THREADS) krylov_combine_kernel(int64_t n, int nvec, int in_planes,
+                                                                    const double *const *__restrict__ v,
+                                                                    const double *__restrict__ coef,
+                                                                    double *__restrict__ out) {
+    __shared__ double c[2 * KC_MAX_VEC];
+    __shared__ const double *vp[KC_MAX_VEC];
+    for (int t = threadIdx.x; t < 2 * nvec; t += blockDim.x) c[t] = coef[t];
+    for (int t = threadIdx.x; t < nvec; t += blockDim.x) vp[t] = v[t];
+    __syncthreads();
+    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    double re = 0.0, im = 0.0;
+    if (in_planes == 2) {
+        for (int k = 0; k < nvec; ++k) {
+            const double xr = vp[k][j], xi = vp[k][n + j], cr = c[2 * k], ci = c[2 * k + 1];
+            re = fma(cr, xr, re);
+            re = fma(-ci, xi, re);
+            im = fma(cr, xi, im);
+            im = fma(ci, xr, im);
+        }
+    } else {
+        for (int k = 0; k < nvec; ++k) {
+            const double x = vp[k][j];
+            re = fma(c[2 * k], x, re);
+            im = fma(c[2 * k + 1], x, im);
+        }
+    }
+    out[j] = re;
+    out[n + j] = im;
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -275,6 +311,30 @@ extern "C" int b200_dot_segments_f64(int64_t n_seg, const int64_t *seg_dev, int6
     dot_seg_kernel<<<grid, B1_THREADS, 0, (cudaStream_t)stream>>>(seg_dev, X, Y, scratch);
     B200_CHECK_LAUNCH();
     dot_final_kernel<<<1, B1_THREADS, 0, (cudaStream_t)stream>>>((int)(gx * n_seg), scratch, out);
+    B200_CHECK_LAUNCH();
+    return B200_OK;
+}
+
+extern "C" int b200_krylov_combine_f64(int64_t n, int64_t nvec, int64_t in_planes, const double *const *V_dev,
+                                       const double *const *V_host, const double *coef_dev, double *OUT,
+                                       b200_stream_t stream) {
+    if (nvec < 1 || nvec > KC_MAX_VEC) return set_error(B200_ERR_ARG, "krylov_combine: nvec = %lld outside 1..%d",
+                                                        (long long)nvec, KC_MAX_VEC);
+    if (in_planes != 1 && in_planes != 2)
+        return set_error(B200_ERR_ARG, "krylov_combine: in_planes = %lld (1 or 2)", (long long)in_planes);
+    if (n < 0) return set_error(B200_ERR_ARG, "krylov_combine: n = %lld < 0", (long long)n);
+    if (n == 0) return B200_OK;
+    if (!V_dev || !V_host || !coef_dev || !OUT) return set_error(B200_ERR_ARG, "krylov_combine: null pointer");
+    const uintptr_t o0 = (uintptr_t)OUT, o1 = o0 + (uintptr_t)(2 * n) * sizeof(double);
+    for (int64_t k = 0; k < nvec; ++k) {
+        const uintptr_t v0 = (uintptr_t)V_host[k], v1 = v0 + (uintptr_t)(in_planes * n) * sizeof(double);
+        if (!V_host[k]) return set_error(B200_ERR_ARG, "krylov_combine: vector %lld is null", (long long)k);
+        if (v0 < o1 && o0 < v1) return set_error(B200_ERR_ARG, "krylov_combine: out overlaps vector %lld", (long long)k);
+    }
+    const int64_t blocks = (n + B1_THREADS - 1) / B1_THREADS;
+    if (blocks > 0x7fffffffLL) return set_error(B200_ERR_ARG, "krylov_combine: n = %lld too large", (long long)n);
+    krylov_combine_kernel<<<(unsigned)blocks, B1_THREADS, 0, (cudaStream_t)stream>>>(n, (int)nvec, (int)in_planes,
+                                                                                     V_dev, coef_dev, OUT);
     B200_CHECK_LAUNCH();
     return B200_OK;
 }

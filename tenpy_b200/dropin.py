@@ -25,6 +25,8 @@ reference engine through the reference's own hook, the class attribute ``Effecti
 ``Sweep.EffectiveH``): :func:`fast_two_site_engine` returns a subclass of the reference's ``TwoSiteDMRGEngine`` whose
 ``EffectiveH`` inherits the reference's ``TwoSiteH`` and the engine's split-order routes
 (:class:`tenpy_b200.algorithms.mps_common.SplitOrderMatvec`, the same code the engine's own ``TwoSiteH`` runs).
+:func:`fast_tdvp_engine` plugs the same effective Hamiltonian and the engine's Lanczos time evolution into the
+reference's TDVP engines.
 """
 import importlib
 import importlib.abc
@@ -32,7 +34,7 @@ import importlib.util
 import os
 import sys
 
-__all__ = ['install', 'installed', 'reference_path', 'fast_two_site_engine']
+__all__ = ['install', 'installed', 'reference_path', 'fast_two_site_engine', 'fast_tdvp_engine']
 
 _ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -95,31 +97,77 @@ def install(path=None):
     return path
 
 
+B200TwoSiteH = None          # the drop-in effective Hamiltonian, made on first use by _two_site_h() (after install())
+
+
+def _two_site_h():
+    """:data:`B200TwoSiteH`: the reference's ``TwoSiteH`` (same constructor, attributes, `combine_theta`, `update_LP` ...)
+    whose `matvec` applies ``LP``, ``W0 W1``, ``RP`` to the split theta without the identity components of the
+    environments where that is cheaper (`SplitOrderMatvec`), the reference order otherwise.  One class, shared by the
+    DMRG and the TDVP engines of this module; it derives from the reference's class, so it is made once the reference is
+    importable."""
+    global B200TwoSiteH
+    if B200TwoSiteH is None:
+        from tenpy.algorithms import mps_common as ref_common
+        from .algorithms.mps_common import SplitOrderMatvec
+
+        class _B200TwoSiteH(SplitOrderMatvec, ref_common.TwoSiteH):
+            """reference ``TwoSiteH`` with the split-order routes of `SplitOrderMatvec` in `matvec`"""
+
+            def __init__(self, env, i0, combine=False, move_right=True):
+                super().__init__(env, i0, combine, move_right)
+                self._H_mpo = env.H
+
+            def matvec(self, theta):
+                # real and complex theta and MPOs alike (SplitOrderMatvec)
+                if self.combine and self._use_split(theta):
+                    return self._matvec_split(theta, theta.get_leg_labels())
+                return super().matvec(theta)
+
+        _B200TwoSiteH.__name__ = _B200TwoSiteH.__qualname__ = 'B200TwoSiteH'
+        B200TwoSiteH = _B200TwoSiteH
+    return B200TwoSiteH
+
+
 def fast_two_site_engine():
     """The reference's ``TwoSiteDMRGEngine`` with the device-optimised effective Hamiltonian plugged in at the reference's
     own extension point ``EffectiveH``.  Call after :func:`install`."""
     if not installed():
         raise RuntimeError('call tenpy_b200.dropin.install() first')
     from tenpy.algorithms import dmrg as ref_dmrg
-    from tenpy.algorithms import mps_common as ref_common
-    from .algorithms.mps_common import SplitOrderMatvec
-
-    class B200TwoSiteH(SplitOrderMatvec, ref_common.TwoSiteH):
-        """reference ``TwoSiteH`` (same constructor, attributes, `combine_theta`, `update_LP` ...); `matvec` applies
-        ``LP``, ``W0 W1``, ``RP`` to the split theta without the identity components of the environments where that is
-        cheaper (`SplitOrderMatvec`), the reference order otherwise."""
-
-        def __init__(self, env, i0, combine=False, move_right=True):
-            super().__init__(env, i0, combine, move_right)
-            self._H_mpo = env.H
-
-        def matvec(self, theta):
-            # real and complex theta and MPOs alike (SplitOrderMatvec)
-            if self.combine and self._use_split(theta):
-                return self._matvec_split(theta, theta.get_leg_labels())
-            return super().matvec(theta)
 
     class B200TwoSiteDMRGEngine(ref_dmrg.TwoSiteDMRGEngine):
-        EffectiveH = B200TwoSiteH
+        EffectiveH = _two_site_h()
 
     return B200TwoSiteDMRGEngine
+
+
+def fast_tdvp_engine(single_site=False):
+    """The reference's ``TwoSiteTDVPEngine`` (or ``SingleSiteTDVPEngine``) with the engine's Lanczos time evolution
+    (:class:`tenpy_b200.linalg.krylov_based.LanczosEvolution`: device-resident scalars, one kernel for the result) in
+    `_krylov_evolve` when ``lanczos_params['hermitian']`` is true (the default; otherwise the reference's own
+    evolution runs), and for two sites the effective Hamiltonian of :func:`fast_two_site_engine`.  Call after
+    :func:`install`."""
+    if not installed():
+        raise RuntimeError('call tenpy_b200.dropin.install() first')
+    import numpy as np
+    from tenpy.algorithms import tdvp as ref_tdvp
+    from .linalg.krylov_based import LanczosEvolution
+    base = ref_tdvp.SingleSiteTDVPEngine if single_site else ref_tdvp.TwoSiteTDVPEngine
+
+    class B200TDVPEngine(base):
+        def _krylov_evolve(self, H, theta, dt):
+            params = self.lanczos_params
+            if not params.get('hermitian', True, bool):
+                return super()._krylov_evolve(H, theta, dt)
+            normalize = params.get('normalize', None)
+            opts = params.as_dict()
+            params.touch(*opts)
+            if np.dtype(H.dtype).kind == 'c' and np.dtype(theta.dtype).kind != 'c':
+                theta = theta.astype(np.complex128)      # a real state, a complex H: the vectors stay packed
+            return LanczosEvolution(H, theta, opts).run(dt, normalize=normalize)
+
+    if not single_site:
+        B200TDVPEngine.EffectiveH = _two_site_h()
+    B200TDVPEngine.__name__ = B200TDVPEngine.__qualname__ = 'B200' + base.__name__
+    return B200TDVPEngine

@@ -1,7 +1,7 @@
-"""Lanczos ground state search on device-resident Arrays.
+"""Lanczos ground state search and time evolution on device-resident Arrays.
 
 Host-side mirror of the reference ``tenpy/linalg/krylov_based.py`` (class `LanczosGroundState` :584,
-`KrylovBased` :30): same options (`N_min`, `N_max`, `P_tol`, `E_tol`, `min_gap`, `N_cache`, `reortho`,
+`LanczosEvolution` :718, `KrylovBased` :30): same options (`N_min`, `N_max`, `P_tol`, `E_tol`, `min_gap`, `N_cache`, `reortho`,
 `cutoff`, `E_shift`), same three-term recurrence, same convergence test (`_converged` :677) and same
 result assembly (`_calc_result_full` :160).  The control flow and the tridiagonal ``eigh`` (at most
 ``(N_max+1)^2`` numbers) stay on the host, as in the reference; every vector operation is a kernel over the
@@ -18,7 +18,7 @@ from .. import backend
 
 logger = logging.getLogger(__name__)
 
-__all__ = ['KrylovBased', 'LanczosGroundState', 'lanczos']
+__all__ = ['KrylovBased', 'LanczosGroundState', 'LanczosEvolution', 'lanczos']
 
 DEVICE_SCALARS_DEFAULT = True    # Lanczos option `device_scalars`: (alpha, beta) stay on the device, read back in chunks
 
@@ -316,6 +316,97 @@ class LanczosGroundState(KrylovBased):
             E_kr, v_kr = np.linalg.eigh(h[:k + 1, :k + 1])
             self.Es[k, :k + 1] = E_kr
             self._result_krylov = v_kr[:, 0]
+
+
+class LanczosEvolution(LanczosGroundState):
+    """``expm(delta H) psi0`` for a hermitian `H` by Lanczos (reference krylov_based.py:718).
+
+    The recurrence is the one of :class:`LanczosGroundState` (on the device-scalar route :meth:`_build_krylov_device`,
+    which replays :meth:`_calc_result_krylov` / :meth:`_converged` below on the host and stops at the ``k`` the reference
+    stops at); ``_h_krylov`` stays real.  In the Krylov basis the result is ``expm(delta h) e_0``, converged when its
+    last component is below `P_tol`.  On the device-scalar route the result ``sum_k c_k v_k`` with complex ``c_k`` is
+    assembled from the cached vectors by ONE kernel (``b200_krylov_combine_f64``; a real start vector gives a complex
+    result) and normalised on the device; the conditioning test is deferred to :meth:`norm_check` as for the ground
+    state.  Otherwise (vectors on different block tables, ``N_cache < N_max``, `reortho`) the host-scalar assembly of
+    :meth:`KrylovBased._calc_result_full` runs.  Options as for :class:`LanczosGroundState`; `E_tol` and `min_gap` are
+    ignored."""
+
+    def __init__(self, H, psi0, options):
+        super().__init__(H, psi0, options)
+        self._result_norm = 1.
+        self.delta = None            # set in run()
+        self._on_device = False      # the last recurrence ran on the device-scalar route
+
+    def run(self, delta, normalize=None):
+        """Returns ``(psi_f, N)``: ``psi_f`` approximates ``expm(delta H) psi0``, normalised if `normalize` (default:
+        ``Re(delta) == 0``), else with the norm ``|psi0| |expm(delta h) e_0|`` (reference krylov_based.py:757)."""
+        self.delta = delta
+        N = self._build_krylov()
+        if N == 1:
+            result_full = self._result_krylov[0] * self.psi0            # _result_krylov[0] is only a phase
+        else:
+            result_full = self._calc_result_full(N)
+        if normalize is None:
+            normalize = np.real(delta) == 0.
+        if normalize:
+            return result_full, N
+        scale = float(self._psi0_norm * self._result_norm)
+        kbuf = getattr(result_full, '_kbuf', None)
+        if kbuf is not None:
+            backend.get_lib().scal(kbuf.numel(), scale, kbuf)
+            return result_full, N
+        return scale * result_full, N
+
+    def _build_krylov_device(self):
+        N = super()._build_krylov_device()
+        self._on_device = N is not None
+        return N
+
+    def _calc_result_full(self, N):
+        """``psi_f = sum_k result_krylov[k] psi[k]`` (reference krylov_based.py:160) in one kernel on the device-scalar
+        route: the terms in the reference's order (``psi[0]``, then the cache from its end), the result packed
+        ``[re | im]`` (:func:`_pack`) and normalised without a host round trip."""
+        cache = self._cache
+        if not self._on_device or len(cache) != N:
+            return super()._calc_result_full(N)
+        order = [0] + list(range(N - 1, 0, -1))
+        v0 = cache[0]
+        packed = getattr(v0, '_kbuf', None) is not None
+        lay = v0.re._layout if packed else v0._layout
+        n = lay.size
+        vf = np.asarray(self._result_krylov, dtype=np.complex128)[order]
+        coef = np.empty(2 * N, dtype=np.float64)
+        coef[0::2], coef[1::2] = vf.real, vf.imag
+        ptrs = np.array([_flat(cache[k])[1].data_ptr() for k in order], dtype=np.int64)
+        lib = backend.get_lib()
+        out = backend.empty(2 * n)
+        lib.krylov_combine(n, 2 if packed else 1, ptrs, backend.to_device(ptrs), backend.to_device(coef), out)
+        self._cache = []
+        psif = npc._from_planes(v0.legs, v0.qtotal, lay, (out[:n], out[n:]), v0.get_leg_labels())
+        psif._kbuf = out
+        n2 = backend.empty(1)
+        lib.dot(2 * n, out, out, backend.dot_scratch(), n2)
+        lib.scal_rsqrt_dev(2 * n, n2, out)
+        self._result_norm2_dev = n2
+        return psif
+
+    def _calc_result_krylov(self, k):
+        """``expm(delta h) e_0`` for ``h = _h_krylov[:k+1, :k+1]``, normalised (reference krylov_based.py:797)."""
+        h = self._h_krylov
+        delta = self.delta
+        if k == 0:
+            exp_dE = np.exp(delta * h[0, 0])
+            self._result_norm = np.abs(exp_dE)
+            self._result_krylov = np.array([exp_dE / self._result_norm])
+        else:
+            E_kr, v_kr = np.linalg.eigh(h[:k + 1, :k + 1])
+            exp_dH_e0 = np.dot(v_kr, np.exp(E_kr * delta) * np.conj(v_kr[0, :]))
+            self._result_norm = np.linalg.norm(exp_dH_e0)
+            self._result_krylov = exp_dH_e0 / self._result_norm
+
+    def _converged(self, k):
+        """Reference krylov_based.py:821."""
+        return np.abs(self._result_krylov[k]) < self.P_tol
 
 
 def lanczos(H, psi, options={}):

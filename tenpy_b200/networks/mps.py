@@ -87,11 +87,13 @@ class MPS:
         self._S[i + 1] = S
 
     def set_B(self, i, B, form='B'):
+        """Reference mps.py:2939; `form` as for `get_B`, e.g. ``'Th'`` for the one-site wave function the TDVP leaves on
+        a site between two updates."""
         self.form[i] = self._to_valid_form(form)
         self._B[i] = B.itranspose(self._B_labels)
 
-    def _scale_axis_B(self, B, S, form_diff, axis_B):
-        """Reference mps.py:5964."""
+    def _scale_axis_B(self, B, S, form_diff, axis_B, cutoff=1e-16):
+        """Reference mps.py:5964; `cutoff`: of the pseudo-inverse of a 2-D `S`."""
         if form_diff == 0.:
             return B
         if not isinstance(S, npc.Array):
@@ -101,7 +103,7 @@ class MPS:
                 S = S**form_diff
             return B.scale_axis(S, axis_B)
         if form_diff == -1.:
-            S = npc.pinv(S, 1e-16)
+            S = npc.pinv(S, cutoff)
         elif form_diff != 1.:
             raise ValueError("Can't scale/tensordot a 2D `S` for non-integer `form_diff`")
         if axis_B == 'vL':
@@ -112,7 +114,7 @@ class MPS:
             B2.ireplace_label(B2.rank - 1, 'vR')
         return B2
 
-    def get_B(self, i, form='B', copy=False, label_p=None):
+    def get_B(self, i, form='B', copy=False, cutoff=1e-16, label_p=None):
         """Tensor of site `i` in the requested canonical form (reference mps.py:2882)."""
         new_form = self._to_valid_form(form)
         old_form = self.form[i]
@@ -124,22 +126,23 @@ class MPS:
                 raise ValueError('can not convert a tensor without canonical form')
             fL, fR = new_form
             if fL is not None and fL != old_form[0]:
-                B = self._scale_axis_B(B, self.get_SL(i), fL - old_form[0], 'vL')
+                B = self._scale_axis_B(B, self.get_SL(i), fL - old_form[0], 'vL', cutoff)
             if fR is not None and fR != old_form[1]:
-                B = self._scale_axis_B(B, self.get_SR(i), fR - old_form[1], 'vR')
+                B = self._scale_axis_B(B, self.get_SR(i), fR - old_form[1], 'vR', cutoff)
         if label_p is not None:
             B = B.replace_label('p', 'p' + label_p)
         return B
 
-    def get_theta(self, i, n=2, formL=1., formR=1.):
-        """n-site wave function with labels ``vL, p0, ..., p{n-1}, vR`` (reference mps.py:3041)."""
+    def get_theta(self, i, n=2, cutoff=1e-16, formL=1., formR=1.):
+        """n-site wave function with labels ``vL, p0, ..., p{n-1}, vR`` (reference mps.py:3041); `cutoff`: of the
+        pseudo-inverse of a 2-D bond matrix."""
         if n == 1:
-            return self.get_B(i, (1., 1.), True, '0')
-        theta = self.get_B(i, (formL, None), False, '0')
+            return self.get_B(i, (1., 1.), True, cutoff, '0')
+        theta = self.get_B(i, (formL, None), False, cutoff, '0')
         old_fR = self.form[i][1]
         for k in range(1, n):
             new_fR = None if k + 1 < n else formR
-            B = self.get_B(i + k, (1. - old_fR, new_fR), False, str(k))
+            B = self.get_B(i + k, (1. - old_fR, new_fR), False, cutoff, str(k))
             old_fR = self.form[i + k][1]
             theta = npc.tensordot(theta, B, axes=['vR', 'vL'])
         return theta
